@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- paired reads/s of the `kallisto quant` hot path on B200 (BASELINE.json metric).
+"""bench.py -- paired reads/s of the `kallisto quant` hot path on an H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 Workload (config.workload): BASELINE config 2 -- a human-GENCODE-v44-like transcriptome index
 (built by the unmodified reference `kallisto index`, k=31; synthetic stand-in, see benchdata.py)
@@ -15,12 +15,21 @@ table is finalised and the EM is run ONCE, inside the timed region (it is part o
            host-buffer figure of the C ABI is listed under config.pinned_host_buffers;
   roofline  = match_kernel: algorithmic bytes (SURVEY.md 8d / DESIGN.md) / CUDA-event time, vs
            MEASURED_PEAKS.json hbm_gbs;
-  --impl reference = oracle/_ref/kallisto (the unmodified reference, built from /root/reference by
+  --impl reference = oracle/_ref/kallisto (the unmodified reference, built from its sources by
            oracle/Makefile) `quant -t <best>` on the SAME FASTQ files (all K x P pairs of rank 0's job, one
            run, process wall clock); cpu_baseline = that run when it happened on this box, else a 2 M-pair sample.
+  --dump-outputs DIR = after the timed runs, what the last timed job handed its caller, as DIR/<name>.npy
+           (float64): est_counts and eff_lens of the EM, and per EC its count and set size (a fixed, seeded sample
+           of the targets / ECs, with their ids, when there are more than DUMP_MAX_ROWS; at most 48 MB in all).
+           The reads are derived from fixed seeds, so two builds run with the same arguments can be compared
+           output for output.  Only the default `quant` workload.
 Every step uses different reads and each batch (pairs_per_step x 200 B) is larger than L2.
+The workload (index, FASTQ files) is cached in the system's temporary directory (shared memory for the FASTQ files),
+never in the source tree, under a name with the user id and a digest of benchdata.py: a cache of another user or of
+another version of the generator is never reused.
 """
 import argparse
+import hashlib
 import json
 import os
 import re
@@ -36,7 +45,10 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 import benchdata  # noqa: E402
 
-DATA = os.path.join(ROOT, "bench_data")
+with open(benchdata.__file__, "rb") as _f:
+    CACHE_TAG = "%d_%s" % (os.getuid(), hashlib.sha256(_f.read()).hexdigest()[:12])
+DATA = os.path.join(tempfile.gettempdir(), "kb_bench_data_" + CACHE_TAG)
+DUMP_MAX_ROWS = 1000000          # per dumped array: 6 arrays x 8 B x 1 M = 48 MB at most
 READ_LEN = 100
 
 
@@ -45,7 +57,7 @@ def log(*a):
 
 
 # ---------------------------------------------------------------------------------------------
-# workload: index + transcriptome (cached under bench_data/, rebuilt with the reference if absent)
+# workload: index + transcriptome (cached under DATA, rebuilt with the reference if absent)
 # ---------------------------------------------------------------------------------------------
 def workload(genes):
     import fcntl
@@ -71,7 +83,7 @@ def workload(genes):
 def _build_workload(genes, idx, txf):
     if not (os.path.exists(idx) and os.path.exists(txf)):
         from oracle import oracle as O
-        log("building workload for %d genes (one-off, cached in bench_data/)" % genes)
+        log("building workload for %d genes (one-off, cached in %s)" % (genes, DATA))
         t0 = time.time()
         tx = benchdata.make_transcriptome(genes, seed=44)
         codes = np.zeros(256, np.uint8)
@@ -88,13 +100,14 @@ def _build_workload(genes, idx, txf):
             with tempfile.TemporaryDirectory(dir=DATA) as td:
                 fa = os.path.join(td, "tx.fa")
                 tx.write_fasta(fa)
-                O.ref_run(["index", "-t", str(min(32, os.cpu_count() or 8)), "-i", idx + ".tmp", fa])
+                # -T: the reference's scratch directory defaults to ./tmp, and the working directory may be read-only
+                O.ref_run(["index", "-t", str(min(32, os.cpu_count() or 8)), "-T", os.path.join(td, "tmp"), "-i", idx + ".tmp", fa])
             os.replace(idx + ".tmp", idx)
         log("workload built in %.0f s" % (time.time() - t0))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -145,7 +158,7 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-CACHE_ROOT = os.path.join("/dev/shm" if os.path.isdir("/dev/shm") else DATA, "kb_bench_cache")
+CACHE_ROOT = os.path.join("/dev/shm", "kb_bench_cache_" + CACHE_TAG) if os.path.isdir("/dev/shm") else os.path.join(DATA, "kb_bench_cache")
 
 
 def job_seeds(rank, W, K):
@@ -255,7 +268,7 @@ def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not measured)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -309,6 +322,25 @@ def reference_sample(idx, files, repeats=1):
                 t_total=round(dt, 2))
 
 
+def dump_outputs(d, em, ec_counts, ec_sizes):
+    """The arrays the timed job returned: est_counts / eff_lens per target, count / size per EC (EC ids in order of
+    first occurrence, so they line up between builds).  More than DUMP_MAX_ROWS targets or ECs: the same seeded sample
+    of ids for both arrays of that kind, written next to them (target_ids / ec_ids)."""
+    os.makedirs(d, exist_ok=True)
+    out = {}
+    for kind, arrays in (("target", {"est_counts": em["est_counts"], "eff_lens": em["eff_lens"]}),
+                         ("ec", {"ec_counts": ec_counts, "ec_sizes": ec_sizes})):
+        n = len(next(iter(arrays.values())))
+        if n > DUMP_MAX_ROWS:
+            ids = np.sort(np.random.default_rng(12345).choice(n, DUMP_MAX_ROWS, replace=False))
+            arrays = {k: a[ids] for k, a in arrays.items()}
+            arrays[kind + "_ids"] = ids
+        out.update(arrays)
+    for name, a in out.items():
+        np.save(os.path.join(d, name + ".npy"), np.asarray(a, np.float64))
+    log("outputs of the last timed job written to %s: %s" % (d, ", ".join(sorted(out))))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -319,6 +351,8 @@ def main():
     ap.add_argument("--genes", type=int, default=int(os.environ.get("KB_BENCH_GENES", "62000")))
     ap.add_argument("--pairs-per-step", type=int, default=int(os.environ.get("KB_BENCH_PAIRS", "2000000")))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed job to DIR/<name>.npy (float64)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -329,6 +363,8 @@ def main():
     workload_name = ("human-GENCODE-v44-like synthetic transcriptome (%d genes, seed 44; reference-built k=31 index), "
                      "synthetic 2x100bp pairs" % args.genes)
     if args.workload != "quant":
+        if args.dump_outputs:
+            ap.error("--dump-outputs is implemented for --workload quant only")
         import bench_extra
         return bench_extra.main(args, rank, world, local_rank, workload_name)
 
@@ -467,6 +503,8 @@ def main():
         eo, et, ec, _ = mc.ec_table()
         ln = np.diff(eo.astype(np.int64))
         em_shape = {"n_ecs": int(len(ln)), "n_multi_ecs": int((ln > 1).sum()), "nnz_multi": int(ln[ln > 1].sum())}
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, em, ec, ln)
     mc.close()
 
     # ---- pinned host buffers through the C ABI, H2D inside (host wall clock) ----
@@ -510,12 +548,6 @@ def main():
                        "bytes_per_round": b_round, "rounds": em["rounds"], "us_per_round": tm["em_ms"] * 1e3 / max(1, em["rounds"]),
                        "note": "the problem lives in L2: bound by the L2 gather rate and the grid barriers of a round, not by HBM",
                        **em_shape}
-    prof = os.path.join(ROOT, "profiles", "match_kernel_traffic.json")
-    if os.path.exists(prof):
-        try:
-            roofline["traffic"] = json.load(open(prof))["dram_bytes_per_launch"]
-        except Exception:
-            pass
 
     # ---- e2e: the drop-in command line, FASTQ files -> abundance.tsv, process wall clock (rank 0 drives all N GPUs
     #      through --devices; the other ranks wait on the host) ----
@@ -569,7 +601,7 @@ def main():
         "ms_per_step": t_total_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "u64/f64", "data": "synthetic",
         "config": {"workload": workload_name, "pairs_per_step": P, "read_len": READ_LEN, "parallelism": "dp%d" % world,
-                   "l2": "every step reads a different %d MB batch (> 126 MB L2)" % (P * 2 * READ_LEN // 1000000),
+                   "l2": "every step reads a different %d MB batch (> 50 MB L2)" % (P * 2 * READ_LEN // 1000000),
                    "em_in_timed_region": True, "align_ms": t_align_ms, "total_ms": t_total_ms,
                    "total_ms_runs": [round(x, 3) for x in runs], "reported_run": "second of two timed runs of the whole job "
                    "(after W warm-up steps and one untimed job)", "untimed_job_ms": round(w_total, 3),

@@ -1,5 +1,5 @@
 """bench.py --workload bus10xv3 | bootstrap: BASELINE configs 3 and 4 (SURVEY.md 8d).  Same JSON contract as the
-quant workload (bench.py); run by hand / from profiles/capture scripts, the driver's default run is `quant`.
+quant workload (bench.py); run by hand; the default run of bench.py is `quant`.
 
   bus10xv3   `kallisto bus -x 10xv3` record path: R1 = 16-nt barcode + 12-nt UMI, R2 = 91-nt cDNA, synthetic
              (benchdata.TorchSimulator10x), human-like index.  step = one batch of read sets through kb_bus_batch_device
@@ -184,7 +184,7 @@ def bus_main(args, local_rank, workload_name):
         cpu = json.load(open(rl))["cpu_baseline"]
     line = {"metric": "read sets/sec bus 10xv3", "value": value, "unit": "reads/s", "n_gpus": 1, "steps": K, "warmup": W,
             "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u64", "data": "synthetic",
-            "config": {"workload": name, "sets_per_step": P, "l2": "every step reads a different %d MB batch (> 126 MB L2)" % (P * (28 + CDNA) // 1000000),
+            "config": {"workload": name, "sets_per_step": P, "l2": "every step reads a different %d MB batch (> 50 MB L2)" % (P * (28 + CDNA) // 1000000),
                        "total_ms_runs": [round(x, 3) for x in runs], "reported_run": "second of two timed runs", "records": n_rec,
                        "p_pseudoaligned": st["n_pseudoaligned"] / max(1, st["n_processed"]), "n_ecs": st["n_ecs"],
                        "resolve_ms_per_launch": tm["resolve_ms"] / max(1, tm["resolve_launches"])},

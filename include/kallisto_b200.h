@@ -1,4 +1,4 @@
-/* kallisto_b200 -- C ABI of the B200-native `kallisto quant` / `kallisto bus` hot path.
+/* kallisto_b200 -- C ABI of the H100-native `kallisto quant` / `kallisto bus` hot path.
  *
  * kallisto (the reference, /root/reference) has no plugin or FFI layer: the hot path sits between
  * its CLI, its index file and its output files (SURVEY.md section 8b).  This header is the boundary a

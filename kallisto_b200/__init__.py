@@ -1,6 +1,6 @@
 """kallisto_b200 -- host-side Python mirror of the C ABI (include/kallisto_b200.h).
 
-The product is the shared library ``libkallisto_b200.so`` (hand-written sm_100a CUDA behind an
+The product is the shared library ``libkallisto_b200.so`` (hand-written sm_90a CUDA behind an
 ``extern "C"`` boundary) and the ``kallisto_b200`` command-line binary; this module is the thin
 ctypes binding used by the tests and ``bench.py``.  Class and method names follow the reference
 objects they stand in for: ``KmerIndex`` (src/KmerIndex.h), ``MinCollector``/``MasterProcessor``

@@ -54,8 +54,8 @@ struct Options {
   std::vector<std::string> files;
 };
 
-// Outputs are written and flushed: leave without tearing down the CUDA context, the 34 GB table and the pinned rings
-// one by one (0.3-0.5 s of a 2-3 s run).  KB_CLI_CLEANUP=1 keeps the orderly release (sanitizer runs).
+// Outputs are written and flushed: leave without tearing down the CUDA context, the k-mer table and the pinned rings
+// one by one (a noticeable share of a short run).  KB_CLI_CLEANUP=1 keeps the orderly release (sanitizer runs).
 [[noreturn]] void finish(int code) {
   std::cout.flush();
   cerr.flush();
@@ -83,7 +83,7 @@ std::string to_json(const std::string& id, const std::string& val, bool quote, b
 }
 
 void usage_quant() {
-  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (B200 build)" << endl
+  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (H100 build)" << endl
             << "Computes equivalence classes for reads and quantifies abundances" << endl << endl
             << "Usage: kallisto_b200 quant [arguments] FASTQ-files" << endl << endl
             << "Required arguments:" << endl
@@ -971,7 +971,7 @@ void write_index_saved(const std::string& in_path, const std::string& out_path, 
 }
 
 void usage_bus() {
-  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (B200 build)" << endl
+  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (H100 build)" << endl
             << "Generates BUS files for single-cell sequencing" << endl << endl
             << "Usage: kallisto_b200 bus [arguments] FASTQ-files" << endl << endl
             << "Required arguments:" << endl
@@ -1386,7 +1386,7 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
 // (-g/-G), priors, --long, -T and bootstraps are refused loudly.
 // ------------------------------------------------------------------------------------------------
 void usage_tcc() {
-  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (B200 build)" << endl
+  std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (H100 build)" << endl
             << "Quantifies abundance from pre-computed transcript-compatibility counts" << endl << endl
             << "Usage: kallisto_b200 quant-tcc [arguments] transcript-compatibility-counts-file" << endl << endl
             << "Required arguments:" << endl

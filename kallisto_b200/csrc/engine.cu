@@ -163,8 +163,8 @@ std::unique_ptr<Index> Index::load(const std::string& path, int device, bool loa
   if (ix->empty_ec != 0xFFFFFFFFu) ix->empty_ec = (uint32_t)ix->h_ec_handle[ix->empty_ec];
 
   // k-mer table.  Every probe costs one random 32-byte sector whatever the table size, and the sector rate of the
-  // L2-miss path is the bound of match_kernel (profiles/README.md), so HBM capacity is traded for shorter probe
-  // sequences: slots >= 4 x k-mers (load 0.14-0.27: 1.14 visits per lookup; human: 34 GB of the 180 GB) when that
+  // L2-miss path is the bound of match_kernel (tools/randbench), so HBM capacity is traded for shorter probe
+  // sequences: slots >= 4 x k-mers (load 0.14-0.27: 1.14 visits per lookup) when that
   // leaves three quarters of the free device memory to the run, else 2 x (load <= 0.5; 1.37 visits measured at
   // 0.27).  KB_TABLE_FACTOR overrides.
   double factor = 4.0;
@@ -177,13 +177,13 @@ std::unique_ptr<Index> Index::load(const std::string& path, int device, bool loa
   if (const char* s = getenv("KB_TABLE_FACTOR")) { const double v = atof(s); if (v >= 1.25 && v <= 64.0) factor = v; }
   ix->table_cap = pow2_ge(std::max<uint64_t>(1024, (uint64_t)((double)f.n_kmers * factor)));
   ix->slots.alloc(ix->table_cap);
-  // presence filter: 2^KB_FILTER_LOG2 bits (default: about 3.5 bits per k-mer, at most 2^29 bits = 64 MB so that it
-  // fits the persisting part of the 126 MB L2; 0 = off).  Single hash: a miss passes it with probability
+  // presence filter: 2^KB_FILTER_LOG2 bits (default: about 3.5 bits per k-mer, at most 2^28 bits = 32 MB so that it
+  // fits the persisting part of the H100's 50 MB L2; 0 = off).  Single hash: a miss passes it with probability
   // 1 - exp(-n / bits).
   uint32_t filter_bits = 0;
   {
     int lg = 0;
-    while ((1ull << lg) < f.n_kmers * 3 && lg < 29) ++lg;
+    while ((1ull << lg) < f.n_kmers * 3 && lg < 28) ++lg;
     if (lg < 16) lg = 16;
     if (const char* s = getenv("KB_FILTER_LOG2")) lg = atoi(s);
     if (lg >= 10 && lg <= 32) filter_bits = lg == 32 ? 0 : (1u << lg);
@@ -1290,11 +1290,17 @@ std::vector<int> Quant::run_bootstrap_device(const std::vector<double>& fl_trunc
     w.bs_counts.download(samples_out->data(), samples_out->size(), 0, st);
     KB_CK(cudaStreamSynchronize(st));
   }
-  // the B problems, `chunk` at a time: alpha + norm + counts of a chunk are meant to stay in L2 next to the shared matrices
+  // the B problems, `chunk` at a time: alpha + norm + counts of a chunk are meant to stay in L2 next to the shared
+  // matrices, so a chunk's vectors take at most half of the device's L2 (25 MB on an H100)
   int chunk = B;
   {
     const size_t per = ((size_t)T + n_multi) * 8 + (size_t)nE * 4;
-    const size_t budget = 64u << 20;
+    int l2 = 0;
+    if (cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, ix_.device) != cudaSuccess || l2 <= 0) {
+      cudaGetLastError();
+      l2 = 50 << 20;
+    }
+    const size_t budget = (size_t)l2 / 2;
     chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)B, budget / std::max<size_t>(1, per)));
     if (const char* s = getenv("KB_BS_CHUNK")) { const int v = atoi(s); if (v > 0) chunk = std::min(B, v); }   // tuning knob
   }

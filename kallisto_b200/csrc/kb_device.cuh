@@ -1,4 +1,4 @@
-// Device-side data layout shared by the kallisto_b200 CUDA kernels (sm_100a).
+// Device-side data layout shared by the kallisto_b200 CUDA kernels (sm_90a).
 //
 // Everything the per-read pseudoalignment loop of the reference touches through
 // pointer-rich host structures (CompactedDBG<Node>::find -> UnitigMap, Node::ec BlockArray,

@@ -25,9 +25,7 @@
 #endif
 #ifndef KB_LOOKAHEAD
 // Experiment (off): inside a run of misses fetch the presence-filter bits of the next KB_LOOKAHEAD k-mers together.
-// Measured slower than one k-mer per iteration (2 / 4 / 8: 1.52 / 1.57 / 1.93 ms against 1.44 ms per 2 M pairs,
-// profiles/match_lookahead_r02.log): the kernel is bound by instruction issue at 12 of 32 lanes active, and the
-// extra hashes cost more than the saved iterations.
+// The extra hashes cost instruction issue in a kernel that runs with few lanes active.
 #define KB_LOOKAHEAD 0
 #endif
 
@@ -45,33 +43,11 @@ __device__ __forceinline__ int32_t ld_relaxed_s32(const int32_t* p) {
   asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-// One 256-bit read-only load (LDG.E.256 on sm_100a): a whole k-mer slot, half a packed read, or a
-// block of memo entries per instruction.  The address must be 32-byte aligned.
+// One 32-byte read-only load as two 128-bit loads (sm_90a has no 256-bit global load): a whole
+// k-mer slot, half a packed read, or a block of memo entries.  The address must be 32-byte aligned,
+// so both halves fall in the same 32-byte sector and the probe still costs one sector of traffic.
 __device__ __forceinline__ void ld256_nc(const void* p, uint32_t (&w)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
-               : "l"(p));
-}
-// The k-mer table probe: one random 32-byte sector out of a multi-GB table, never reused.
-#ifndef KB_PROBE_LD
-#define KB_PROBE_LD 0
-#endif
-__device__ __forceinline__ void ld256_probe(const void* p, uint32_t (&w)[8]) {
-#if KB_PROBE_LD == 0
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-#elif KB_PROBE_LD == 1
-  asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-#elif KB_PROBE_LD == 2
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-#elif KB_PROBE_LD == 3
   asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8]; ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
-#elif KB_PROBE_LD == 4
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-#elif KB_PROBE_LD == 5
-  asm volatile("ld.global.cg.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-#elif KB_PROBE_LD == 6
-  asm volatile("ld.global.cg.v4.b32 {%0,%1,%2,%3}, [%8]; ld.global.cg.v4.b32 {%4,%5,%6,%7}, [%8+16];"
-#endif
                : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                : "l"(p));
 }
@@ -309,8 +285,8 @@ __global__ void __launch_bounds__(256) dlist_scan_kernel(DevIndex ix, BatchArgs 
 // (unmappable read: every k-mer is probed).  As straight-line per-thread code a warp pays the
 // maximum over its lanes, and lanes sitting at different call sites serialise.  Here each lane
 // keeps an explicit state and every iteration of the warp's loop performs exactly ONE lookup per
-// active lane through a single convergent site: canonical k-mer + hash, one LDG.E.256 of the
-// 32-byte slot, then the reference's control flow as a state transition
+// active lane through a single convergent site: canonical k-mer + hash, one 32-byte load of the
+// slot (two 128-bit loads of the same sector on sm_90a), then the reference's control flow as a state transition
 //   MAIN     the k-mer at p.  Miss: next valid k-mer.  Hit: record it, distance to the end of its EC
 //            block (1780-1788); if >= 2 go to JUMP.
 //   JUMP     the jump target (1793-1827).  Absent or same (unitig, EC set): accepted, scanning resumes
@@ -527,7 +503,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
       }
       __syncwarp();
       // ---- refill: the idle lanes take the next fragments of the warp's chunk and copy their packed
-      //      reads (pack_kernel output) into shared memory with 256-bit loads
+      //      reads (pack_kernel output) into shared memory with 32-byte loads (ld256_nc)
       {
         const bool is_idle = (idle >> lane) & 1u;
         const uint32_t rank = __popc(idle & ((1u << lane) - 1));
@@ -645,7 +621,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
       }
       uint32_t v[8];
       if (!absent) {
-        ld256_probe(ix.slots + slot, v);
+        ld256_nc(ix.slots + slot, v);
         pv += 0x10000u;
       } else {
         v[0] = v[1] = 0xFFFFFFFFu;     // reads as an empty slot: a miss
@@ -1106,7 +1082,7 @@ void launch_pseudoalign(const DevIndex& ix, const DevDict& dd, const BatchArgs& 
   if (ev) cudaEventRecord(ev[1], st);
   match_kernel<<<blocks, tpb, smem, st>>>(ix, dd, ba);
   if (ev) cudaEventRecord(ev[2], st);
-  switch (ra.group) {      // lanes per fragment (engine.cu: KB_RESOLVE_G, default 32: profiles/resolve_group_sweep_r02.jsonl)
+  switch (ra.group) {      // lanes per fragment (engine.cu: KB_RESOLVE_G, default 32)
     case 4: resolve_kernel<4><<<(ra.n_warps * 4 + 127) / 128, 128, 0, st>>>(ix, dd, ba, ra); break;
     case 8: resolve_kernel<8><<<(ra.n_warps * 8 + 127) / 128, 128, 0, st>>>(ix, dd, ba, ra); break;
     case 16: resolve_kernel<16><<<(ra.n_warps * 16 + 127) / 128, 128, 0, st>>>(ix, dd, ba, ra); break;

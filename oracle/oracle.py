@@ -9,6 +9,7 @@ import gzip
 import os
 import struct
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -230,11 +231,17 @@ def have_ref():
 
 
 def ref_run(args, cwd=None, check=True):
-    return subprocess.run([REF_BIN] + list(args), cwd=cwd, check=check, stdout=subprocess.PIPE, stderr=subprocess.PIPE)
+    r = subprocess.run([REF_BIN] + list(args), cwd=cwd, stdout=subprocess.PIPE, stderr=subprocess.PIPE)
+    if check and r.returncode != 0:
+        raise RuntimeError("%s %s failed (exit %d): %s" % (REF_BIN, " ".join(map(str, args)), r.returncode,
+                                                          r.stderr.decode(errors="replace")[-600:]))
+    return r
 
 
 def ref_index(fasta, out, k=31, threads=1):
-    ref_run(["index", "-i", out, "-k", str(k), "-t", str(threads), fasta])
+    # the reference's scratch directory (-T) defaults to ./tmp: keep it out of the working directory
+    with tempfile.TemporaryDirectory() as td:
+        ref_run(["index", "-i", out, "-k", str(k), "-t", str(threads), "-T", os.path.join(td, "tmp"), fasta])
     return out
 
 

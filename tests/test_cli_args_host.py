@@ -1,16 +1,18 @@
 """CPU: option validation of the kallisto_b200 command line against the unmodified reference binary
 (CheckOptionsEM / CheckOptionsBus, src/main.cpp:1283-1805): same exit code and the same `Error:` lines for
-invocations that are rejected before any device work.  Skipped where oracle/_ref/kallisto is not built."""
+invocations that are rejected before any device work.  The reference's exit codes and `Error:` lines are stored in
+tests/golden/cli_args.json (written by `python tests/golden/make_golden.py cli_args`)."""
+import json
 import os
 import subprocess
 
 import pytest
 
-from oracle import oracle as O
 from tests import util
 
 BIN = os.path.join(util.ROOT, "kallisto_b200", "kallisto_b200")
-pytestmark = pytest.mark.skipif(not (O.have_ref() and os.path.exists(BIN)), reason="needs oracle/_ref/kallisto and the CLI")
+GOLD = os.path.join(util.GOLDEN, "cli_args.json")
+pytestmark = pytest.mark.skipif(not os.path.exists(BIN), reason="needs the CLI")
 
 D = os.path.join(util.GOLDEN, "config1")
 IDX, R1, R2 = (os.path.join(D, f) for f in ("transcripts.kidx", "reads_1.fastq.gz", "reads_2.fastq.gz"))
@@ -60,11 +62,20 @@ def errors(binary, args, cwd):
     return r.returncode, [l.strip() for l in r.stderr.splitlines() if l.startswith("Error")]
 
 
+def case_key(args):
+    """Arguments of a case, with the repository's directory written as <ROOT>"""
+    return " ".join(a.replace(util.ROOT, "<ROOT>") for a in args)
+
+
+def reference_errors(args):
+    with open(GOLD) as f:
+        rc, lines = json.load(f)[case_key(args)]
+    return rc, [l.replace("<ROOT>", util.ROOT) for l in lines]
+
+
 @pytest.mark.parametrize("args", CASES, ids=lambda a: " ".join(os.path.basename(x) for x in a)[:60])
 def test_rejected_like_the_reference(args, tmp_path):
-    (tmp_path / "a").mkdir()
-    (tmp_path / "b").mkdir()
-    want = errors(O.REF_BIN, args, str(tmp_path / "a"))
-    got = errors(BIN, args, str(tmp_path / "b"))
+    want = reference_errors(args)
+    got = errors(BIN, args, str(tmp_path))
     assert want[0] != 0, "the reference accepts this invocation: not a validation case"
     assert got == want

@@ -53,8 +53,8 @@ def test_export_import_equals_single_run(name):
 
 
 def test_nccl_merge_with_one_rank_is_the_identity():
-    """kb_comm_create / kb_quant_merge_nccl on a one-rank communicator (what the driver's one-GPU box can run; the
-    N-rank exchange is checked by tools/multi_check.py under torchrun, see profiles/)."""
+    """kb_comm_create / kb_quant_merge_nccl on a one-rank communicator (what a one-GPU machine can run; the
+    N-rank exchange is checked by tools/multi_check.py under torchrun)."""
     ds = util.dataset("synth_small")
     ix = K.KmerIndex(ds["index"], device=0)
     a = K.MinCollector(ix, paired=True)

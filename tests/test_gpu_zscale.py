@@ -1,6 +1,6 @@
-"""GPU: parity at BASELINE config-2 scale -- the 62 000-gene / 147 M-k-mer index the benchmark uses (34 GB k-mer
-table, 711 k index EC sets, 45 k short unitigs), >= 2 M synthetic 2x100 bp pairs, against the UNMODIFIED reference
-(oracle/_ref/kallisto) run on the same FASTQ files on this box's host cores:
+"""GPU: parity at BASELINE config-2 scale -- the 62 000-gene / 147 M-k-mer index the benchmark uses (711 k index
+EC sets, 45 k short unitigs; a 2^29-slot = 17 GB k-mer table on an 80 GB H100), >= 2 M synthetic 2x100 bp pairs, against
+the UNMODIFIED reference (oracle/_ref/kallisto) run on the same FASTQ files on the host cores:
 
   * per-fragment equivalence classes: `kallisto bus -x bulk --paired --num -t 1` (main.cpp:1050-1107,
     ProcessReads.cpp:1643-1701) on 8 consecutive slices of the input in parallel processes; every fragment's

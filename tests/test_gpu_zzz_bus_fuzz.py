@@ -1,8 +1,7 @@
 """GPU: the CUDA BUS path (kb_bus_create / kb_bus_batch) on the random technology layouts of tests/test_oracle_bus_fuzz.py
 -- barcode / UMI pieces anywhere, with and without UMI, one sequence read or a pair with random start offsets, tag
 sequences, strand modes, --num, too-short reads, Ns -- against the BUS record model, which the CPU suite holds to the
-unmodified reference binary on the very same cases.  (Written after the round's GPU budget was spent: first run is the
-driver's.)"""
+unmodified reference on the very same cases."""
 import numpy as np
 import pytest
 
@@ -12,7 +11,7 @@ from tests.test_oracle_bus_fuzz import layout
 from tests.test_oracle_bus_paired import sorted_records
 from tests.test_oracle_fuzz import make_case
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not O.have_ref(), reason="the random indices are built by oracle/_ref/kallisto")]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("seed", range(8))

@@ -1,7 +1,8 @@
-"""CPU: the oracle (oracle/kb_oracle.cpp) against the UNMODIFIED reference binary (oracle/_ref/kallisto) on small
-random transcriptomes that are generated on the fly -- other k, shared exons, short transcripts, Ns, read lengths
-around k.  Strengthens the pin of the oracle beyond the committed fixtures; skipped where the reference binary is
-not present (it is built by `make -C oracle` from /root/reference and travels to the GPU box with the snapshot)."""
+"""CPU: the oracle (oracle/kb_oracle.cpp) against the UNMODIFIED reference (oracle/_ref/kallisto) on small random
+transcriptomes -- other k, shared exons, short transcripts, Ns, read lengths around k.  Strengthens the pin of the
+oracle beyond the committed fixtures.  The transcriptomes and reads are generated here from their seeds; the index the
+reference built for each one and the reference's per-fragment ECs, matrix.ec and flens.txt for each case are stored
+under tests/golden/fuzz (written by `python tests/golden/make_golden.py fuzz`)."""
 import os
 
 import numpy as np
@@ -10,12 +11,18 @@ import pytest
 from oracle import oracle as O
 from tests import util
 
-pytestmark = pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref/kallisto not built")
-
+FUZZ = os.path.join(util.GOLDEN, "fuzz")
 COMP = bytes.maketrans(b"ACGT", b"TGCA")
 
 
-def make_case(tmp, seed, k, read_len, n_reads):
+def case_index(seed, k):
+    """The reference's index of the transcriptome of make_case(seed, k)."""
+    return os.path.join(FUZZ, "s%d_k%d.kidx" % (seed, k))
+
+
+def make_case(tmp, seed, k, read_len, n_reads, build_index=None):
+    """Transcriptome (written to tmp/t.fa) and reads of one case; build_index(fasta, out, k) re-creates the stored
+    index with the reference (tests/golden/make_golden.py)."""
     rng = np.random.default_rng(seed)
     lut = np.frombuffer(b"ACGT", np.uint8)
     exons = [bytes(lut[rng.integers(0, 4, int(rng.integers(k + 3, 220)))]) for _ in range(24)]
@@ -32,7 +39,9 @@ def make_case(tmp, seed, k, read_len, n_reads):
     with open(fa, "wb") as f:
         for i, t in enumerate(txs):
             f.write(b">tx%d\n%s\n" % (i, t))
-    idx = O.ref_index(fa, os.path.join(tmp, "t.kidx"), k=k)
+    idx = case_index(seed, k)
+    if build_index:
+        build_index(fa, idx, k=k)
     r1, r2 = [], []
     for _ in range(n_reads):
         t = txs[int(rng.integers(0, len(txs)))]
@@ -64,17 +73,29 @@ def make_case(tmp, seed, k, read_len, n_reads):
     return idx, r1, r2, paths
 
 
-@pytest.mark.parametrize("seed,k,read_len", [(1, 31, 75), (2, 21, 50), (3, 15, 36), (4, 31, 33), (5, 27, 150)])
-@pytest.mark.parametrize("mode", ["paired", "single", "paired_fr", "single_rf"])
-def test_random_transcriptome(seed, k, read_len, mode, tmp_path):
-    paired = mode.startswith("paired")
+def reference_ecs(seed, mode):
+    """-> (per-fragment EC id or -1, EC sets, flens or None) of `kallisto bus -x bulk --num -t 1` on the case."""
+    z = np.load(os.path.join(FUZZ, "s%d_%s.npz" % (seed, mode)))
+    flens = z["flens"] if "flens" in z.files else None
+    return z["frag_ec"].astype(np.int64), util.ec_sets(z["ec_off"], z["ec_tids"]), flens
+
+
+def mode_args(mode):
+    """-> (paired, strand code of the oracle, strand option of the reference)"""
     strand = {"fr": 1, "rf": 2}.get(mode.split("_")[-1], 0)
-    extra = {0: [], 1: ["--fr-stranded"], 2: ["--rf-stranded"]}[strand]
+    return mode.startswith("paired"), strand, {0: [], 1: ["--fr-stranded"], 2: ["--rf-stranded"]}[strand]
+
+
+CASES = [(1, 31, 75), (2, 21, 50), (3, 15, 36), (4, 31, 33), (5, 27, 150)]
+MODES = ["paired", "single", "paired_fr", "single_rf"]
+
+
+@pytest.mark.parametrize("seed,k,read_len", CASES)
+@pytest.mark.parametrize("mode", MODES)
+def test_random_transcriptome(seed, k, read_len, mode, tmp_path):
+    paired, strand, _ = mode_args(mode)
     idx, r1, r2, paths = make_case(str(tmp_path), seed, k, read_len, 1500)
-    rec, ecs, flens = O.ref_ec_dump(idx, str(tmp_path / "o"), paths if paired else paths[:1], paired=paired, extra=extra)
-    n = len(r1)
-    want = np.full(n, -1, np.int64)
-    want[rec["flags"]] = rec["ec"]
+    want, ecs, flens = reference_ecs(seed, mode)
 
     ix = O.OracleIndex(idx)
     run = O.OracleRun(ix, paired, strand, True)
@@ -82,6 +103,6 @@ def test_random_transcriptome(seed, k, read_len, mode, tmp_path):
     got = run.pseudoalign(bases, off)
     eo, et, ec = run.ec_table()
     np.testing.assert_array_equal(got, want)
-    assert util.ec_sets(eo, et) == [tuple(e) for e in ecs]
+    assert util.ec_sets(eo, et) == ecs
     if paired and flens is not None:
         np.testing.assert_array_equal(run.flens(), flens)

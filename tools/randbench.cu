@@ -1,8 +1,8 @@
-// Microbenchmark: how many independent random 32-byte sector reads per second does a B200 sustain
+// Microbenchmark: how many independent random 32-byte sector reads per second does the GPU sustain
 // over a table of a given size?  This is the hardware ceiling for the k-mer table probes of
 // match_kernel (one random sector per probe, no reuse), as opposed to the streaming-copy bandwidth
 // in MEASURED_PEAKS.json.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/randbench tools/randbench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/randbench tools/randbench.cu
 //   tools/randbench [table_GiB ...]          (RB_FULL=1: also dependent chains, 32-byte L2 fetch granularity,
 //                                             64/128-byte accesses; RB_VMM=1: table mapped with cuMemCreate/cuMemMap)
 #include <cstdint>
@@ -17,7 +17,7 @@ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
   return x;
 }
 __device__ __forceinline__ void ld256(const void* p, uint32_t (&w)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8]; ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
 }
 
