@@ -323,7 +323,7 @@ def bootstrap_main(args, local_rank, workload_name):
             "gpu_launches": int(kl),
             "roofline": {"bound": "hbm", "kernel": "em_kernel (batched)", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None,
                          "peak_source": peak_src, "traffic": None,
-                         "note": "the batched EM works out of L2 (chunks of samples sized to 64 MB of alpha/norm/counts); see roofline_em of the quant line"}}
+                         "note": "the batched EM works out of L2 (chunks of samples whose alpha/norm/counts take at most half of the L2); see roofline_em of the quant line"}}
     rl = os.path.join(d, "reference_bs_line.json")
     if os.path.exists(rl):
         ref = json.load(open(rl))

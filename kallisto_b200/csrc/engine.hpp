@@ -199,10 +199,6 @@ class Quant {
   EmResult run_em(const EcTable& ecs, const std::vector<double>& fl_trunc, int max_iter = 10000, int min_rounds = 50);
   // Same result, EC table built and kept on the device (the `quant` fast path).
   EmResult run_em_device(const std::vector<double>& fl_trunc, int max_iter = 10000, int min_rounds = 50);
-  // B bootstrap EMs (Bootstrap::run_em): alpha_out is B x n_targets.  Returns rounds per bootstrap.
-  std::vector<int> run_bootstrap(const EcTable& ecs, const std::vector<double>& fl_trunc, uint64_t seed, int B,
-                                 std::vector<double>& alpha_out, std::vector<uint32_t>* samples_out = nullptr);
-
   // ---- multi-GPU: ship this rank's equivalence classes to another rank / fold another rank's in ----
   // export_prepare numbers the ECs (first occurrence) and lays the table out on the device; returns
   // {n_sets, n_entries}.  export_copy then fills caller-provided DEVICE buffers (e.g. torch tensors

@@ -143,7 +143,12 @@ struct EmProblem {
   // (quant-tcc: the weights are the SAMPLE's counts / eff_len, src/weights.cpp:220-246)
   uint64_t w_stride;
 };
-int em_max_blocks(int threads_per_block);
+// Most problems one launch_em may carry: em_kernel keeps an int of state per problem in dynamic shared memory (32 KB
+// here, under the 48 KB a launch gets without opting in).  The bootstrap and quant-tcc also launch their resample /
+// fill kernels for at most this many samples at a time: the samples sit on gridDim.y (at most 65 535).
+static constexpr int KB_EM_MAX_BATCH = 8192;
+// co-resident blocks of em_kernel for `nb` problems (the cooperative launch's limit)
+int em_max_blocks(int threads_per_block, int nb);
 // quant-tcc helpers: dense per-sample count vectors from the sparse TCC rows, and per-sample weights in CSR and CSC order
 struct TccFill {
   uint32_t n_ec, n_targets, nb;        // samples in this chunk

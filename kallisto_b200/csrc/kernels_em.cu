@@ -279,12 +279,12 @@ SingleShape em_single_shape() {
 }
 }  // namespace
 
-int em_max_blocks(int tpb) {
+int em_max_blocks(int tpb, int nb) {
   int dev = 0, sms = 0, per_sm = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int t = tpb >= 1024 ? 1024 : (tpb >= 512 ? 512 : 256);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, em_fn(t, em_occ()), t, 4096);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, em_fn(t, em_occ()), t, (size_t)nb * sizeof(int));
   return sms * per_sm;
 }
 
@@ -308,7 +308,7 @@ void launch_em(const EmProblem& p, int tpb_req, cudaStream_t st) {
     return;
   }
   const int tpb = tpb_req >= 1024 ? 1024 : (tpb_req >= 512 ? 512 : 256);
-  const int maxb = em_max_blocks(tpb);
+  const int maxb = em_max_blocks(tpb, p.nb);
   const uint64_t work = (uint64_t)p.nb * (p.n_multi > p.n_targets ? p.n_multi : p.n_targets);
   int blocks = (int)((work + tpb - 1) / tpb);
   if (blocks > maxb) blocks = maxb;
