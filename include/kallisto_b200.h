@@ -197,6 +197,19 @@ int kb_bootstrap_run(kb_quant* q, double fld_mean, double fld_sd, uint64_t seed,
 int kb_tcc_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
                const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
                int32_t per_sample_eff, double* est_counts_out, int32_t* rounds_out);
+/* Bootstraps of quant-tcc (src/main.cpp:3109-3178): n_bootstrap per sample, each the sample's counts resampled
+ * (Multinomial::sample with the seeds of mt19937_64(seed), the same seeds for every sample) and run through the EM with
+ * the sample's ORIGINAL counts / eff_len as weights.  Problem g = sample * n_bootstrap + b.  The results are handed to
+ * `cb` in chunks, in order: problems first .. first + count - 1, est_counts (count x n_targets, row-major), rounds
+ * (count) and, when want_samples != 0, the resampled counts (count x n_ecs); the pointers are valid during the call
+ * only.  A non-zero return from cb stops the run (KB_ERR_INVALID).  Arguments as kb_tcc_run, except that the EC ids
+ * of a row must be strictly increasing; a row's total count must fit an int32. */
+typedef int (*kb_tcc_bootstrap_cb)(void* user, uint64_t first, uint32_t count, const double* est_counts,
+                                   const int32_t* rounds, const uint32_t* samples);
+int kb_tcc_bootstrap_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                         const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                         int32_t per_sample_eff, uint64_t seed, int32_t n_bootstrap, int32_t want_samples,
+                         kb_tcc_bootstrap_cb cb, void* user);
 /* mean_fl_trunc -> eff_lens exactly as the reference forms them (get_frag_len_means + calc_eff_lens, src/weights.cpp:7-28,
  * 58-79): fld_mean > 0: truncated Gaussian (-l/-s); else the histogram flens[1000]; both 0/NULL: eff_len = 1 for every
  * target (quant-tcc without fragment-length information).  Host arithmetic. */

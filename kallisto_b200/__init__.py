@@ -99,8 +99,12 @@ EXPORTED_SYMBOLS = [
     "kb_quant_get_timings", "kb_quant_finalize", "kb_quant_ec_table", "kb_quant_get_flens",
     "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
     "kb_comm_unique_id", "kb_comm_create", "kb_comm_create_from_nccl", "kb_comm_create_all", "kb_comm_reserve", "kb_comm_free",
-    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
+    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
 ]
+
+# kb_tcc_bootstrap_cb: (user, first problem, count, est_counts, rounds, resampled counts or NULL) -> 0 to go on
+TCC_BOOTSTRAP_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(C.c_double), C.POINTER(C.c_int32),
+                               C.POINTER(C.c_uint32))
 
 _lib = None
 
@@ -158,6 +162,7 @@ def lib():
     L.kb_quant_set_frag_base.argtypes = [vp, u64]
     L.kb_quant_reserve.argtypes = [vp, u64, u64]
     L.kb_tcc_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, vp]
+    L.kb_tcc_bootstrap_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, u64, i32, i32, TCC_BOOTSTRAP_CB, vp]
     L.kb_eff_lens.argtypes = [vp, vp, dbl, dbl, vp, C.POINTER(dbl), C.POINTER(dbl)]
     L.kb_bus_create.argtypes = [vp, C.POINTER(kb_bus_opts), C.POINTER(vp)]
     L.kb_bus_batch.argtypes = [vp, vp, vp, u32, vp, C.POINTER(u32)]
@@ -518,6 +523,35 @@ def tcc_run(index, ec_sets, rows, eff):
     _ck(lib().kb_tcc_run(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals), _p(eff), per_sample,
                          _p(est), _p(rounds)))
     return est, rounds[: len(rows)]
+
+
+def tcc_bootstrap(index, ec_off, ec_tids, row_off, ec_ids, counts, eff, seed, n_bootstrap, on_chunk, want_samples=False):
+    """kb_tcc_bootstrap_run on CSR arrays (EC table ec_off / ec_tids, TCC rows row_off / ec_ids / counts, EC ids strictly
+    increasing within a row).  on_chunk(first, est (count, T), rounds (count,), samples (count, n_ecs) or None) receives
+    the problems g = row * n_bootstrap + b in order; the arrays are copies."""
+    T = index.num_trans
+    n_ecs = len(ec_off) - 1
+    ec_off, ro = np.ascontiguousarray(ec_off, np.uint64), np.ascontiguousarray(row_off, np.uint64)
+    ec_tids = np.ascontiguousarray(ec_tids if len(ec_tids) else np.zeros(1), np.uint32)
+    ec_ids = np.ascontiguousarray(ec_ids if len(ec_ids) else np.zeros(1), np.uint32)
+    counts = np.ascontiguousarray(counts if len(counts) else np.zeros(1), np.uint32)
+    eff = np.ascontiguousarray(eff, np.float64)
+    err = []
+
+    def cb(_user, first, count, est, rounds, samples):
+        try:
+            on_chunk(first, np.ctypeslib.as_array(est, (count, T)).copy(), np.ctypeslib.as_array(rounds, (count,)).copy(),
+                     np.ctypeslib.as_array(samples, (count, n_ecs)).copy() if samples and n_ecs else None)
+            return 0
+        except BaseException as e:      # stops the run; raised again below
+            err.append(e)
+            return 1
+    rc = lib().kb_tcc_bootstrap_run(index._h, n_ecs, _p(ec_off), _p(ec_tids), len(ro) - 1, _p(ro), _p(ec_ids), _p(counts),
+                                    _p(eff), int(eff.ndim == 2), int(seed), int(n_bootstrap), int(want_samples),
+                                    TCC_BOOTSTRAP_CB(cb), None)
+    if err:
+        raise err[0]
+    _ck(rc)
 
 
 def fastx_summary(path, threads=1):

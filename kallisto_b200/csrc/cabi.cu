@@ -402,6 +402,25 @@ int kb_tcc_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const u
   });
 }
 
+int kb_tcc_bootstrap_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                         const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                         int32_t per_sample_eff, uint64_t seed, int32_t n_bootstrap, int32_t want_samples,
+                         kb_tcc_bootstrap_cb cb, void* user) {
+  if (!ix || !ec_offsets || !row_offsets || !eff_lens || !cb || (n_ecs && !tids) || n_bootstrap < 0)
+    return fail(KB_ERR_INVALID, "kb_tcc_bootstrap_run: bad argument");
+  return guarded([&] {
+    kb::TccInput in;
+    in.n_ecs = n_ecs; in.ec_off = ec_offsets; in.tids = tids; in.n_samples = n_samples; in.row_off = row_offsets;
+    in.ec_ids = ec_ids; in.counts = counts; in.eff_lens = eff_lens; in.per_sample_eff = per_sample_eff != 0;
+    kb::tcc_bootstrap(*ix->ix, in, seed, n_bootstrap, want_samples != 0,
+                      [&](uint64_t first, uint32_t count, const double* est, const int* rounds, const uint32_t* samples) {
+                        static_assert(sizeof(int) == sizeof(int32_t), "rounds are handed out as int32_t");
+                        if (cb(user, first, count, est, reinterpret_cast<const int32_t*>(rounds), samples) != 0)
+                          throw std::invalid_argument("kb_tcc_bootstrap_run: stopped by the callback");
+                      });
+  });
+}
+
 int kb_eff_lens(const kb_index* ix, const uint32_t* flens, double fld_mean, double fld_sd, double* eff_out, double* mean_out,
                 double* sd_out) {
   if (!ix || !eff_out) return fail(KB_ERR_INVALID, "kb_eff_lens: null argument");

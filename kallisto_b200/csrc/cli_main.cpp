@@ -27,6 +27,9 @@
 #include <vector>
 
 #include "../../include/kallisto_b200.h"
+// Bound weakly: the command line also links against stand-ins of the library that carry only the entry points of the
+// host pipeline (tests/stub); there `quant-tcc -b` reports the missing entry point instead of failing to link.
+#pragma weak kb_tcc_bootstrap_run
 #include "fastx.hpp"
 #include "h5_reader.hpp"
 #include "h5_writer.hpp"
@@ -1381,9 +1384,14 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
 // ------------------------------------------------------------------------------------------------
 // kallisto quant-tcc (src/main.cpp:394-513 ParseOptionsTCCQuant, 1807-1967 CheckOptionsTCCQuant, 2802-3220 body):
 // abundances from pre-computed transcript-compatibility counts.  Every row of the TCC matrix is one EM over the
-// equivalence classes of the EC file; all rows are solved on the device by the batched EM kernel (kb_tcc_run).
-// Supported: -i, -e (required here), -o, -l/-s, -f, -t, --matrix-to-files, --plaintext.  Gene-level output
-// (-g/-G), priors, --long, -T and bootstraps are refused loudly.
+// equivalence classes of the EC file; all rows are solved on the device by the batched EM kernel (kb_tcc_run), and
+// their bootstraps (-b) likewise, every (row, bootstrap) pair its own problem (kb_tcc_bootstrap_run).
+// Supported: -i, -e (required here), -o, -l/-s, -f, -t, -b, -d/--seed, --matrix-to-files, --matrix-to-directories,
+// --plaintext.  Gene-level output (-g/-G), priors, --long, -T and a per-sample abundance.h5 are refused loudly.
+// Deliberate differences from the reference:
+//   - -b on a matrix file without --matrix-to-files / --matrix-to-directories, or without --plaintext, is refused: the
+//     reference (built without HDF5) runs and silently writes no bootstraps there.
+//   - -b on a non-matrix file whose counts are all zero is an error; the reference aborts (Multinomial::sample(0)).
 // ------------------------------------------------------------------------------------------------
 void usage_tcc() {
   std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (H100 build)" << endl
@@ -1399,7 +1407,13 @@ void usage_tcc() {
             << "-l, --fragment-length=DOUBLE  Estimated average fragment length" << endl
             << "-s, --sd=DOUBLE               Estimated standard deviation of fragment length" << endl
             << "-t, --threads=INT             Number of host threads (default: 1)" << endl
+            << "-b, --bootstrap-samples=INT   Number of bootstrap samples (default: 0); with a matrix file only" << endl
+            << "                              together with --matrix-to-files or --matrix-to-directories and --plaintext" << endl
+            << "    --seed=INT                Seed for the bootstrap sampling (default: 42)" << endl
             << "    --matrix-to-files         Reorganize matrix output into abundance tsv files" << endl
+            << "    --matrix-to-directories   Reorganize matrix output into abundance tsv files across" << endl
+            << "                              multiple directories" << endl
+            << "    --plaintext               Output plaintext only (quant-tcc writes no HDF5 in this build)" << endl
             << "    --device=INT              CUDA device ordinal (default: 0)" << endl;
 }
 
@@ -1426,6 +1440,7 @@ int cmd_quant_tcc(int argc, char** argv) {
   std::string index, ecfile, output, fldfile, tccfile, genemap, gtf, priors, txnames;
   double fld = 0.0, sd = 0.0;
   int threads = 1, device = 0, bootstrap = 0;
+  size_t seed = 42;
   int matrix_to_files = 0, matrix_to_dirs = 0, plaintext = 0, long_flag = 0;
   const char* opt_string = "o:i:T:e:f:P:l:s:t:g:G:b:d:p:D:";
   static struct option long_options[] = {{"plaintext", no_argument, &plaintext, 1},
@@ -1461,6 +1476,7 @@ int cmd_quant_tcc(int argc, char** argv) {
       case 'g': genemap = optarg; break;
       case 'G': gtf = optarg; break;
       case 'b': std::stringstream(optarg) >> bootstrap; break;
+      case 'd': std::stringstream(optarg) >> seed; break;
       case 'T': txnames = optarg; break;
       case 'p': priors = optarg; break;
       case 'D': std::stringstream(optarg) >> device; break;
@@ -1468,6 +1484,7 @@ int cmd_quant_tcc(int argc, char** argv) {
     }
   }
   if (optind < argc) tccfile = argv[optind];
+  if (matrix_to_dirs) matrix_to_files = 1;     // --matrix-to-directories implies --matrix-to-files (src/main.cpp:499-502)
   // ---- CheckOptionsTCCQuant
   bool ret = true;
   struct stat stt;
@@ -1486,8 +1503,15 @@ int cmd_quant_tcc(int argc, char** argv) {
   if (!fldfile.empty() && stat(fldfile.c_str(), &stt) != 0) { cerr << ERROR_STR << " fragment length distribution file not found " << fldfile << endl; ret = false; }
   if (!genemap.empty() || !gtf.empty()) { cerr << ERROR_STR << " gene-level output (--genemap / --gtf) is not supported by this build" << endl; ret = false; }
   if (!priors.empty() || long_flag || !txnames.empty()) { cerr << ERROR_STR << " --priors, --long and --txnames are not supported by this build" << endl; ret = false; }
-  if (bootstrap != 0) { cerr << ERROR_STR << " bootstrapping of quant-tcc is not supported by this build" << endl; ret = false; }
-  if (matrix_to_dirs) { cerr << ERROR_STR << " --matrix-to-directories is not supported by this build (use --matrix-to-files)" << endl; ret = false; }
+  if (bootstrap > 0 && (!matrix_to_files || !plaintext) && !tccfile.empty()) {
+    std::ifstream in(tccfile);
+    std::string first;
+    if (getline(in, first) && first.rfind("%%MatrixMarket", 0) == 0) {
+      cerr << ERROR_STR << " bootstraps of a TCC matrix are not supported without --matrix-to-files (or --matrix-to-directories)"
+           << " and --plaintext" << endl;
+      ret = false;
+    }
+  }
   if ((fld != 0.0 || sd != 0.0) && !fldfile.empty()) { cerr << ERROR_STR << " cannot supply mean or sd while also supplying a fragment length distribution file" << endl; ret = false; }
   if ((fld != 0.0 && sd == 0.0) || (sd != 0.0 && fld == 0.0)) { cerr << ERROR_STR << " cannot supply mean/sd without supplying both -l and -s" << endl; ret = false; }
   if (ret && fld > 0.0 && sd > 0.0) cerr << "[tcc] fragment length distribution is truncated gaussian with mean = " << fld << ", sd = " << sd << endl;
@@ -1498,6 +1522,7 @@ int cmd_quant_tcc(int argc, char** argv) {
     if (!S_ISDIR(stt.st_mode)) { cerr << ERROR_STR << " file " << output << " exists and is not a directory" << endl; ret = false; }
   } else if (mkdir(output.c_str(), 0777) == -1) { cerr << ERROR_STR << " could not create directory " << output << endl; ret = false; }
   if (threads <= 0) { cerr << ERROR_STR << " invalid number of threads " << threads << endl; ret = false; }
+  if (bootstrap < 0) { cerr << "Error: number of bootstrap samples must be a non-negative integer." << endl; ret = false; }
   if (!ret) { cerr << endl; usage_tcc(); return 1; }
 
   kb_index* ix = nullptr;
@@ -1612,6 +1637,10 @@ int cmd_quant_tcc(int argc, char** argv) {
     }
     nrow = rows.size();
   }
+  if (bootstrap > 0 && !is_matrix && std::all_of(vals.begin(), vals.end(), [](uint32_t v) { return v == 0; })) {
+    cerr << "Error: cannot bootstrap a TCC file without any counts" << endl;
+    return 1;
+  }
   // ---- effective lengths (src/main.cpp:2998-3028)
   const bool calc_eff = !fldfile.empty() || fld != 0.0;
   std::vector<std::vector<uint32_t>> flds;
@@ -1679,13 +1708,71 @@ int cmd_quant_tcc(int argc, char** argv) {
           tpm_m[r].push_back({(int)i, tpm[i]});
           if (calc_eff) el[r].push_back({(int)i, e[i]});
         }
-      if (matrix_to_files) write_abundance(output + "/abundance_" + std::to_string(r + 1) + ".tsv", names, lens, e, a);
+      if (matrix_to_dirs) {
+        const std::string dir = output + "/abundance_" + std::to_string(r + 1);     // src/main.cpp:3063-3084
+        struct stat ds;
+        if (stat(dir.c_str(), &ds) == 0) {
+          if (!S_ISDIR(ds.st_mode)) { cerr << "Error: file " << dir << " exists and is not a directory" << endl; return 1; }
+        } else if (mkdir(dir.c_str(), 0777) == -1) {
+          cerr << "Error: could not create directory " << dir << endl;
+          return 1;
+        }
+        write_abundance(dir + "/abundance.tsv", names, lens, e, a);
+      } else if (matrix_to_files) {
+        write_abundance(output + "/abundance_" + std::to_string(r + 1) + ".tsv", names, lens, e, a);
+      }
     }
     write_sparse_matrix(output + "/matrix.abundance.mtx", ab, T);
     write_sparse_matrix(output + "/matrix.abundance.tpm.mtx", tpm_m, T);
     if (calc_eff) write_sparse_matrix(output + "/matrix.efflens.mtx", el, T);
   } else {
     write_abundance(output + "/abundance.tsv", names, lens, eff.data(), est.data());
+  }
+  if (bootstrap > 0) {
+    // src/main.cpp:3109-3178: bs_abundance_<b>.tsv (non-matrix file), bs_abundance_<row>_<b>.tsv (--matrix-to-files) or
+    // abundance_<row>/bs_abundance_<b>.tsv (--matrix-to-directories), rows numbered from 1, each written with its row's
+    // eff_lens.  A matrix row without any non-zero estimate gets B copies of that (zero) estimate.  The device hands the
+    // (row, bootstrap) problems over chunk by chunk; up to -t threads write a chunk's files.
+    cerr << "[bstrp] running EM for " << pretty_num((size_t)nrow * bootstrap) << " bootstraps" << endl;
+    std::vector<char> empty_row(nrow, 0);
+    if (is_matrix)
+      for (size_t r = 0; r < nrow; ++r)
+        empty_row[r] = std::none_of(est.begin() + r * T, est.begin() + (r + 1) * T, [](double x) { return x > 0.0; });
+    struct Ctx {
+      const std::string* output;
+      bool is_matrix, dirs, per_sample;
+      int B, threads;
+      uint32_t T;
+      const std::vector<std::string>* names;
+      const std::vector<uint32_t>* lens;
+      const std::vector<double>* eff;
+      const std::vector<double>* est;
+      const std::vector<char>* empty_row;
+    } ctx{&output, is_matrix, matrix_to_dirs != 0, per_sample, bootstrap, threads, T, &names, &lens, &eff, &est, &empty_row};
+    auto write_chunk = [](void* user, uint64_t first, uint32_t count, const double* bs_est, const int32_t*, const uint32_t*) -> int {
+      const Ctx& c = *static_cast<const Ctx*>(user);
+      auto write_one = [&](uint32_t i) {
+        const uint64_t g = first + i, r = g / c.B, b = g % c.B;
+        std::string path;
+        if (!c.is_matrix) path = *c.output + "/bs_abundance_" + std::to_string(b) + ".tsv";
+        else if (c.dirs) path = *c.output + "/abundance_" + std::to_string(r + 1) + "/bs_abundance_" + std::to_string(b) + ".tsv";
+        else path = *c.output + "/bs_abundance_" + std::to_string(r + 1) + "_" + std::to_string(b) + ".tsv";
+        const double* a = (*c.empty_row)[r] ? c.est->data() + r * c.T : bs_est + (size_t)i * c.T;
+        write_abundance(path, *c.names, *c.lens, c.eff->data() + (c.per_sample ? r : 0) * (size_t)c.T, a);
+      };
+      const uint32_t nt = (uint32_t)std::min<int64_t>(c.threads, count);
+      std::vector<std::thread> pool;
+      for (uint32_t t = 1; t < nt; ++t)
+        pool.emplace_back([&, t] { for (uint32_t i = t; i < count; i += nt) write_one(i); });
+      for (uint32_t i = 0; i < count; i += nt) write_one(i);
+      for (auto& th : pool) th.join();
+      return 0;
+    };
+    if (!kb_tcc_bootstrap_run) { cerr << "Error: this libkallisto_b200 has no kb_tcc_bootstrap_run" << endl; return 1; }
+    KB_TRY(kb_tcc_bootstrap_run(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow, row_off.data(),
+                                ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(), eff.data(),
+                                per_sample ? 1 : 0, (uint64_t)seed, bootstrap, 0, write_chunk, &ctx));
+    cerr << " done" << endl << endl;
   }
   if (calc_eff) {
     std::ofstream of(output + "/matrix.fld.tsv");                 // writeFLD, src/PlaintextWriter.cpp:287-298

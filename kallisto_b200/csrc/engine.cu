@@ -1470,58 +1470,101 @@ void Quant::import_sets_device(uint32_t n_sets, const uint32_t* d_off, const uin
   KB_CK(cudaStreamSynchronize(stream_));
 }
 
+namespace {
+struct StreamGuard {    // a private non-blocking stream, destroyed on every way out
+  cudaStream_t s = nullptr;
+  StreamGuard() { KB_CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
+  ~StreamGuard() { if (s) cudaStreamDestroy(s); }
+  StreamGuard(const StreamGuard&) = delete;
+  StreamGuard& operator=(const StreamGuard&) = delete;
+};
+
+// The structure every quant-tcc problem shares, from the EC table (EC ids = line numbers of matrix.ec), on the device:
+// CSR of the multi-transcript ECs, CSC by transcript, singletons, the (EC id, transcript) of every entry that
+// launch_tcc_fill forms the weights from, and the TCC rows themselves.
+struct TccShape {
+  uint64_t nnz = 0;
+  uint32_t n_multi = 0;
+  DBuf<uint32_t> multi_ec, m_off, m_tid, m_ec, t_off, t_midx, t_ec, t_tid, ecid, val;
+  DBuf<int32_t> single;
+
+  TccShape(uint32_t T, const TccInput& in, cudaStream_t st) {
+    const uint32_t nE = in.n_ecs, S = in.n_samples;
+    std::vector<uint32_t> h_multi_ec, h_m_off{0}, h_m_tid, h_m_ec, h_t_off(T + 1, 0), h_t_midx, h_t_ec, h_t_tid;
+    std::vector<int32_t> t_single(T, -1);
+    for (uint32_t e = 0; e < nE; ++e) {
+      const uint64_t b = in.ec_off[e], n = in.ec_off[e + 1] - b;
+      for (uint64_t j = 0; j < n; ++j)
+        if (in.tids[b + j] >= T) throw Error("kallisto_b200: equivalence class file has a transcript id out of range");
+      if (n == 1) { t_single[in.tids[b]] = (int32_t)e; continue; }
+      if (n == 0) continue;
+      h_multi_ec.push_back(e);
+      for (uint64_t j = 0; j < n; ++j) {
+        h_m_tid.push_back(in.tids[b + j]);
+        h_m_ec.push_back(e);
+        ++h_t_off[in.tids[b + j] + 1];
+      }
+      h_m_off.push_back((uint32_t)h_m_tid.size());
+    }
+    nnz = h_m_tid.size();
+    n_multi = (uint32_t)h_multi_ec.size();
+    for (uint32_t t = 0; t < T; ++t) h_t_off[t + 1] += h_t_off[t];
+    h_t_midx.resize(nnz); h_t_ec.resize(nnz); h_t_tid.resize(nnz);
+    {
+      std::vector<uint32_t> fill(h_t_off.begin(), h_t_off.end() - 1);
+      for (uint32_t r = 0; r < n_multi; ++r)
+        for (uint32_t j = h_m_off[r]; j < h_m_off[r + 1]; ++j) {
+          const uint32_t t = h_m_tid[j], at = fill[t]++;
+          h_t_midx[at] = r; h_t_ec[at] = h_multi_ec[r]; h_t_tid[at] = t;
+        }
+    }
+    for (uint64_t i = 0; i < in.row_off[S]; ++i)
+      if (in.ec_ids[i] >= nE) throw Error("kallisto_b200: TCC file refers to an equivalence class that is not in the EC file");
+    auto up32 = [&](DBuf<uint32_t>& d, const std::vector<uint32_t>& h) { d.alloc(std::max<size_t>(1, h.size())); d.upload(h.data(), h.size(), st); };
+    up32(multi_ec, h_multi_ec); up32(m_off, h_m_off); up32(m_tid, h_m_tid); up32(m_ec, h_m_ec);
+    up32(t_off, h_t_off); up32(t_midx, h_t_midx); up32(t_ec, h_t_ec); up32(t_tid, h_t_tid);
+    single.upload(t_single.data(), T, st);
+    ecid.alloc(std::max<uint64_t>(1, in.row_off[S])); ecid.upload(in.ec_ids, in.row_off[S], st);
+    val.alloc(std::max<uint64_t>(1, in.row_off[S])); val.upload(in.counts, in.row_off[S], st);
+    KB_CK(cudaStreamSynchronize(st));     // the host vectors go out of scope
+  }
+  // weights of `nb` rows (row_off: their nb + 1 offsets into ecid / val) into counts / m_w / t_w
+  TccFill fill(uint32_t nE, uint32_t T, int nb, const unsigned long long* row_off, uint32_t* counts, const double* eff,
+               uint64_t eff_stride, double* m_w, double* t_w) const {
+    TccFill f{};
+    f.n_ec = nE; f.n_targets = T; f.nb = (uint32_t)nb; f.row_off = row_off; f.ec_ids = ecid.p; f.vals = val.p;
+    f.counts = counts; f.nnz = nnz; f.m_ec = m_ec.p; f.m_tid = m_tid.p; f.t_ec = t_ec.p; f.t_tid = t_tid.p;
+    f.eff = eff; f.eff_stride = eff_stride; f.m_w = m_w; f.t_w = t_w;
+    return f;
+  }
+  EmProblem problem(uint32_t nE, uint32_t T) const {
+    EmProblem p{};
+    p.n_ec = nE; p.n_targets = T; p.n_multi = n_multi;
+    p.multi_ec = multi_ec.p; p.m_off = m_off.p; p.m_tid = m_tid.p;
+    p.t_off = t_off.p; p.t_midx = t_midx.p; p.t_single = single.p;
+    p.max_iter = 10000; p.min_rounds = 50; p.w_stride = nnz;
+    return p;
+  }
+};
+}  // namespace
+
 std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out) {
   KB_CK(cudaSetDevice(ix.device));
   const uint32_t T = ix.flat.num_targets(), nE = in.n_ecs, S = in.n_samples;
   alpha_out.assign((size_t)S * T, 0.0);
   std::vector<int> rounds(S, 0);
   if (S == 0) return rounds;
-  // structure of the problem on the host, from the EC table (EC ids = line numbers of matrix.ec)
-  std::vector<uint32_t> multi_ec, m_off{0}, m_tid, m_ec, t_off(T + 1, 0), t_midx, t_ec, t_tid;
-  std::vector<int32_t> t_single(T, -1);
-  for (uint32_t e = 0; e < nE; ++e) {
-    const uint64_t b = in.ec_off[e], n = in.ec_off[e + 1] - b;
-    for (uint64_t j = 0; j < n; ++j)
-      if (in.tids[b + j] >= T) throw Error("kallisto_b200: equivalence class file has a transcript id out of range");
-    if (n == 1) { t_single[in.tids[b]] = (int32_t)e; continue; }
-    if (n == 0) continue;
-    multi_ec.push_back(e);
-    for (uint64_t j = 0; j < n; ++j) {
-      m_tid.push_back(in.tids[b + j]);
-      m_ec.push_back(e);
-      ++t_off[in.tids[b + j] + 1];
-    }
-    m_off.push_back((uint32_t)m_tid.size());
-  }
-  const uint64_t nnz = m_tid.size();
-  const uint32_t n_multi = (uint32_t)multi_ec.size();
-  for (uint32_t t = 0; t < T; ++t) t_off[t + 1] += t_off[t];
-  t_midx.resize(nnz); t_ec.resize(nnz); t_tid.resize(nnz);
-  {
-    std::vector<uint32_t> fill(t_off.begin(), t_off.end() - 1);
-    for (uint32_t r = 0; r < n_multi; ++r)
-      for (uint32_t j = m_off[r]; j < m_off[r + 1]; ++j) {
-        const uint32_t t = m_tid[j], at = fill[t]++;
-        t_midx[at] = r; t_ec[at] = multi_ec[r]; t_tid[at] = t;
-      }
-  }
-  for (uint64_t i = 0; i < in.row_off[S]; ++i)
-    if (in.ec_ids[i] >= nE) throw Error("kallisto_b200: TCC file refers to an equivalence class that is not in the EC file");
-  cudaStream_t st = nullptr;
-  KB_CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  DBuf<uint32_t> d_multi_ec, d_m_off, d_m_tid, d_m_ec, d_t_off, d_t_midx, d_t_ec, d_t_tid, d_ecid, d_val, d_counts;
-  DBuf<int32_t> d_single;
+  StreamGuard sg;
+  const cudaStream_t st = sg.s;
+  const TccShape sh(T, in, st);
+  const uint64_t nnz = sh.nnz;
+  const uint32_t n_multi = sh.n_multi;
+  DBuf<uint32_t> d_counts;
   DBuf<unsigned long long> d_rowoff;
   DBuf<double> d_eff, d_mw, d_tw, d_alpha, d_norm, d_single_cnt;
   DBuf<uint32_t> d_cnt_row;
   DBuf<int> d_emi;
   DBuf<unsigned> d_ch, d_bar;
-  auto up32 = [&](DBuf<uint32_t>& d, const std::vector<uint32_t>& h) { d.alloc(std::max<size_t>(1, h.size())); d.upload(h.data(), h.size(), st); };
-  up32(d_multi_ec, multi_ec); up32(d_m_off, m_off); up32(d_m_tid, m_tid); up32(d_m_ec, m_ec);
-  up32(d_t_off, t_off); up32(d_t_midx, t_midx); up32(d_t_ec, t_ec); up32(d_t_tid, t_tid);
-  d_single.upload(t_single.data(), T, st);
-  d_ecid.alloc(std::max<uint64_t>(1, in.row_off[S])); d_ecid.upload(in.ec_ids, in.row_off[S], st);
-  d_val.alloc(std::max<uint64_t>(1, in.row_off[S])); d_val.upload(in.counts, in.row_off[S], st);
   // samples per chunk: weights dominate (16 bytes per entry and sample); ~2 GB of work space
   const size_t per = (size_t)nnz * 16 + (size_t)nE * 4 + ((size_t)T + n_multi) * 8;
   int chunk = (int)std::max<size_t>(1, std::min<size_t>(S, ((size_t)2 << 30) / std::max<size_t>(1, per)));
@@ -1542,23 +1585,16 @@ std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alp
     for (int b = 0; b <= nb; ++b) ro[b] = in.row_off[s0 + b];
     d_rowoff.upload(ro.data(), (size_t)nb + 1, st);
     if (in.per_sample_eff) d_eff.upload(in.eff_lens + (size_t)s0 * T, (size_t)nb * T, st);
-    TccFill f{};
-    f.n_ec = nE; f.n_targets = T; f.nb = (uint32_t)nb; f.row_off = d_rowoff.p; f.ec_ids = d_ecid.p; f.vals = d_val.p;
-    f.counts = d_counts.p; f.nnz = nnz; f.m_ec = d_m_ec.p; f.m_tid = d_m_tid.p; f.t_ec = d_t_ec.p; f.t_tid = d_t_tid.p;
-    f.eff = d_eff.p; f.eff_stride = in.per_sample_eff ? T : 0; f.m_w = d_mw.p; f.t_w = d_tw.p;
-    launch_tcc_fill(f, st);
+    launch_tcc_fill(sh.fill(nE, T, nb, d_rowoff.p, d_counts.p, d_eff.p, in.per_sample_eff ? T : 0, d_mw.p, d_tw.p), st);
     KB_CK(cudaGetLastError());
     launch_fill_f64(d_alpha.p, (uint64_t)nb * T, 1.0 / T, st);
     d_emi.zero(st);
     d_ch.zero(st);
-    EmProblem p{};
-    p.n_ec = nE; p.n_targets = T; p.n_multi = n_multi;
-    p.multi_ec = d_multi_ec.p; p.m_off = d_m_off.p; p.m_tid = d_m_tid.p; p.m_w = d_mw.p;
-    p.t_off = d_t_off.p; p.t_midx = d_t_midx.p; p.t_w = d_tw.p; p.t_single = d_single.p;
+    EmProblem p = sh.problem(nE, T);
+    p.m_w = d_mw.p; p.t_w = d_tw.p;
     p.nb = nb; p.counts = d_counts.p; p.alpha = d_alpha.p; p.norm = d_norm.p;
     p.rounds = d_emi.p; p.fstate = d_emi.p + chunk; p.bar = d_bar.p; p.chcount = d_ch.p;
     p.cnt_row = d_cnt_row.p; p.single_cnt = d_single_cnt.p;
-    p.max_iter = 10000; p.min_rounds = 50; p.w_stride = nnz;
     launch_em(p, em_tpb(), st);
     KB_CK(cudaGetLastError());
     d_alpha.download(alpha_out.data() + (size_t)s0 * T, (size_t)nb * T, 0, st);
@@ -1571,8 +1607,153 @@ std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alp
           if (alpha_out[(size_t)(s0 + b) * T + t] < 1e-7 / 10.0) alpha_out[(size_t)(s0 + b) * T + t] = 0.0;
     }
   }
-  cudaStreamDestroy(st);
   return rounds;
+}
+
+void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool want_samples, const TccBootstrapSink& sink) {
+  KB_CK(cudaSetDevice(ix.device));
+  const uint32_t T = ix.flat.num_targets(), nE = in.n_ecs, S = in.n_samples;
+  if (S == 0 || B <= 0) return;
+  StreamGuard sg;
+  const cudaStream_t st = sg.s;
+  const TccShape sh(T, in, st);      // checks the EC ids
+  const uint64_t nnz = sh.nnz;
+  const uint32_t n_multi = sh.n_multi;
+  // Multinomial::sample of every row (src/Multinomial.hpp): std::discrete_distribution<int> over the row's DENSE counts
+  // (n_ecs of them).  libstdc++ normalises by the sum, takes partial sums in order and sets the LAST dense entry to
+  // 1.0; a draw is the first index whose partial sum is >= u.  The table here keeps the non-zero ECs only, in the same
+  // sequential double arithmetic: a zero count adds 0.0 to the sum and to the partial sum, which changes neither.
+  //   - A zero-count EC e never wins a draw: its partial sum equals that of the EC before it, which comes first in the
+  //     search; for e = 0 it is 0.0, and u > 0 always (generate_canonical over minstd_rand0: u = 0 needs two
+  //     consecutive engine outputs of 1, and 16807 * 1 != 1).  So dropping those entries changes no draw ...
+  //   - ... except for the last EC: its entry is forced to 1.0 even when its count is 0, and a u above the row's last
+  //     partial sum (below 1 by rounding) lands on it.  If EC n_ecs - 1 has count 0 the table ends with a sentinel
+  //     entry (EC n_ecs - 1, 1.0); otherwise the row's own last entry is set to 1.0.
+  // With one EC (n_ecs == 1) libstdc++ keeps no table and returns 0 for every draw; the one-entry table does the same.
+  std::vector<unsigned long long> cp_off(S + 1, 0), n_draws(S, 0);
+  std::vector<double> cp;
+  std::vector<uint32_t> cp_ec;
+  for (uint32_t r = 0; r < S; ++r) {
+    const uint64_t a = in.row_off[r], z = in.row_off[r + 1];
+    double sum = 0.0;
+    uint64_t N = 0;
+    for (uint64_t i = a; i < z; ++i) {
+      if (i > a && in.ec_ids[i] <= in.ec_ids[i - 1])
+        throw Error("kallisto_b200: the EC ids of a TCC row must be strictly increasing for bootstrapping");
+      sum += (double)in.counts[i];
+      N += in.counts[i];
+    }
+    if (N > 2147483647ull) throw Error("kallisto_b200: a TCC row holds more than 2^31 - 1 counts (Multinomial::n_ is an int)");
+    n_draws[r] = N;
+    if (N) {
+      double acc = 0.0;
+      for (uint64_t i = a; i < z; ++i) {
+        if (!in.counts[i]) continue;
+        acc += (double)in.counts[i] / sum;
+        cp.push_back(acc);
+        cp_ec.push_back(in.ec_ids[i]);
+      }
+      if (cp_ec.back() == nE - 1) cp.back() = 1.0;
+      else { cp.push_back(1.0); cp_ec.push_back(nE - 1); }
+    }
+    cp_off[r + 1] = cp.size();
+  }
+  // seeds (src/main.cpp:3125-3130): the same B for every row
+  std::vector<uint32_t> x0(B);
+  {
+    std::mt19937_64 rnd;
+    rnd.seed(seed);
+    for (int b = 0; b < B; ++b) {
+      uint32_t x = (uint32_t)(rnd() % 2147483647ull);   // minstd_rand0 seeding (linear_congruential_engine::seed)
+      if (x == 0) x = 1;
+      x0[b] = x;
+    }
+  }
+  // problems per chunk (a chunk may split a row's B bootstraps): the per-problem vectors plus the weights of the rows the
+  // chunk touches fit ~2 GB of work space
+  const uint64_t P = (uint64_t)S * B;
+  auto rows_of = [&](uint64_t c) { return std::min<uint64_t>(S, (c + B - 2) / B + 1); };   // most rows c problems touch
+  const size_t per_prob = (size_t)nE * 4 + (size_t)T * 16 + (size_t)n_multi * 12 + 32;
+  const size_t per_row = (size_t)nnz * 16 + (size_t)nE * 4 + (in.per_sample_eff ? (size_t)T * 8 : 0) + 16;
+  auto fits = [&](uint64_t c) { return c * per_prob + rows_of(c) * per_row <= ((size_t)2 << 30); };
+  uint64_t chunk = std::min<uint64_t>(P, KB_EM_MAX_BATCH);
+  if (!fits(chunk)) {
+    uint64_t lo = 1, hi = chunk;     // largest chunk that fits (1 if none does)
+    while (hi - lo > 1) { const uint64_t mid = (lo + hi) / 2; if (fits(mid)) lo = mid; else hi = mid; }
+    chunk = lo;
+  }
+  if (const char* s = getenv("KB_TCC_BS_CHUNK")) { const long v = atol(s); if (v > 0) chunk = std::min<uint64_t>(P, v); }   // tests
+  chunk = std::min<uint64_t>(chunk, KB_EM_MAX_BATCH);
+  const uint64_t rmax = rows_of(chunk);
+  DBuf<uint32_t> d_counts, d_samp, d_x0, d_cp_ec, d_wset, d_cnt_row;
+  DBuf<unsigned long long> d_rowoff, d_cp_off, d_ndraws, d_chunkoff;
+  DBuf<double> d_eff, d_mw, d_tw, d_alpha, d_norm, d_single_cnt, d_cp;
+  DBuf<int> d_emi;
+  DBuf<unsigned> d_ch, d_bar;
+  d_counts.alloc(rmax * std::max<uint32_t>(1, nE));
+  d_mw.alloc(std::max<size_t>(1, rmax * nnz)); d_tw.alloc(std::max<size_t>(1, rmax * nnz));
+  d_eff.alloc(in.per_sample_eff ? rmax * T : (size_t)T);
+  if (!in.per_sample_eff) d_eff.upload(in.eff_lens, T, st);
+  d_rowoff.alloc(rmax + 1);
+  d_samp.alloc(chunk * std::max<uint32_t>(1, nE));
+  d_alpha.alloc(chunk * T); d_norm.alloc(std::max<size_t>(1, chunk * n_multi));
+  d_cnt_row.alloc(std::max<size_t>(1, chunk * n_multi)); d_single_cnt.alloc(chunk * T);
+  d_emi.alloc(2 * chunk); d_ch.alloc(2 * chunk); d_bar.alloc(1);
+  d_wset.alloc(chunk); d_chunkoff.alloc(chunk + 1);
+  d_x0.alloc(B); d_x0.upload(x0.data(), B, st);
+  d_cp_off.alloc(S + 1); d_cp_off.upload(cp_off.data(), S + 1, st);
+  d_ndraws.alloc(S); d_ndraws.upload(n_draws.data(), S, st);
+  d_cp.alloc(std::max<size_t>(1, cp.size())); d_cp.upload(cp.data(), cp.size(), st);
+  d_cp_ec.alloc(std::max<size_t>(1, cp_ec.size())); d_cp_ec.upload(cp_ec.data(), cp_ec.size(), st);
+  std::vector<unsigned long long> ro(rmax + 1), coff(chunk + 1);
+  std::vector<uint32_t> wset(chunk), samp(want_samples ? chunk * nE : 0);
+  std::vector<double> est(chunk * T);
+  std::vector<int> emi(2 * chunk);
+  for (uint64_t g0 = 0; g0 < P; g0 += chunk) {
+    const int nb = (int)std::min<uint64_t>(chunk, P - g0);
+    const uint64_t r0 = g0 / B, nr = (g0 + nb - 1) / B - r0 + 1;
+    // the original counts of the chunk's rows -> their weights (calc_weights(tc_.counts, ...), src/weights.cpp:220-246)
+    for (uint64_t i = 0; i <= nr; ++i) ro[i] = in.row_off[r0 + i];
+    d_rowoff.upload(ro.data(), nr + 1, st);
+    if (in.per_sample_eff) d_eff.upload(in.eff_lens + r0 * T, nr * T, st);
+    launch_tcc_fill(sh.fill(nE, T, (int)nr, d_rowoff.p, d_counts.p, d_eff.p, in.per_sample_eff ? T : 0, d_mw.p, d_tw.p), st);
+    KB_CK(cudaGetLastError());
+    // resampled counts
+    coff[0] = 0;
+    for (int i = 0; i < nb; ++i) {
+      const uint64_t r = (g0 + i) / B;
+      wset[i] = (uint32_t)(r - r0);
+      coff[i + 1] = coff[i] + (n_draws[r] + 63) / 64;
+    }
+    d_wset.upload(wset.data(), nb, st);
+    d_chunkoff.upload(coff.data(), (size_t)nb + 1, st);
+    TccResampleArgs ra{};
+    ra.n_ec = nE; ra.nb = (uint32_t)nb; ra.first = g0; ra.B = (uint32_t)B; ra.x0 = d_x0.p;
+    ra.cp_off = d_cp_off.p; ra.cp = d_cp.p; ra.cp_ec = d_cp_ec.p; ra.n_draws = d_ndraws.p;
+    ra.chunk_off = d_chunkoff.p; ra.n_chunks = coff[nb]; ra.samp = d_samp.p;
+    launch_tcc_resample(ra, st);
+    KB_CK(cudaGetLastError());
+    // the EMs: uniform start, weights of the problem's row
+    launch_fill_f64(d_alpha.p, (uint64_t)nb * T, 1.0 / T, st);
+    d_emi.zero(st);
+    d_ch.zero(st);
+    EmProblem p = sh.problem(nE, T);
+    p.m_w = d_mw.p; p.t_w = d_tw.p; p.w_set = d_wset.p;
+    p.nb = nb; p.counts = d_samp.p; p.alpha = d_alpha.p; p.norm = d_norm.p;
+    p.rounds = d_emi.p; p.fstate = d_emi.p + chunk; p.bar = d_bar.p; p.chcount = d_ch.p;
+    p.cnt_row = d_cnt_row.p; p.single_cnt = d_single_cnt.p;
+    launch_em(p, em_tpb(), st);
+    KB_CK(cudaGetLastError());
+    d_alpha.download(est.data(), (size_t)nb * T, 0, st);
+    d_emi.download(emi.data(), 2 * chunk, 0, st);
+    if (want_samples) d_samp.download(samp.data(), (size_t)nb * nE, 0, st);
+    KB_CK(cudaStreamSynchronize(st));
+    for (int b = 0; b < nb; ++b)
+      if (emi[chunk + b] == 3)   // stop detected on the last allowed iteration: zero small alphas (EMAlgorithm.h:213-216)
+        for (uint32_t t = 0; t < T; ++t)
+          if (est[(size_t)b * T + t] < 1e-7 / 10.0) est[(size_t)b * T + t] = 0.0;
+    sink(g0, (uint32_t)nb, est.data(), emi.data(), want_samples ? samp.data() : nullptr);
+  }
 }
 
 template struct DBuf<uint8_t>;

@@ -10,6 +10,7 @@
 // without a CUDA device every entry point throws.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -318,5 +319,11 @@ struct TccInput {
   bool per_sample_eff = false;
 };
 std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out /* n_samples x n_targets */);
+// The B bootstraps of every sample (src/main.cpp:3109-3178), problem g = sample * B + b, handed to `sink` chunk by chunk
+// in order: (first problem, count, est_counts count x n_targets, rounds, resampled counts count x n_ecs or nullptr).
+// Host memory is bounded by one chunk, whatever n_samples x B.
+using TccBootstrapSink = std::function<void(uint64_t first, uint32_t count, const double* est, const int* rounds,
+                                            const uint32_t* samples)>;
+void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool want_samples, const TccBootstrapSink& sink);
 
 }  // namespace kb

@@ -142,6 +142,9 @@ struct EmProblem {
   // 0: the weights m_w / t_w are shared by all problems (quant, bootstrap); nnz: problem b has its own at [b * w_stride]
   // (quant-tcc: the weights are the SAMPLE's counts / eff_len, src/weights.cpp:220-246)
   uint64_t w_stride;
+  // optional, with w_stride != 0: problem b reads weight set w_set[b] instead of set b (quant-tcc bootstrap: the B
+  // resampled problems of a row share that row's weights).  nullptr: set b.
+  const uint32_t* w_set;
 };
 // Most problems one launch_em may carry: em_kernel keeps an int of state per problem in dynamic shared memory (32 KB
 // here, under the 48 KB a launch gets without opting in).  The bootstrap and quant-tcc also launch their resample /
@@ -256,5 +259,24 @@ struct ResampleArgs {
   uint32_t* samp;            // nb x n_ec output counts (zeroed by the launcher)
 };
 void launch_resample(const ResampleArgs& a, cudaStream_t st);
+
+// quant-tcc bootstrap: problem p of a launch is global problem g = first + p, i.e. bootstrap g % B of row g / B.  Every
+// row has a cumulative table over its NON-ZERO ECs (plus the sentinel of the last EC, see tcc_bootstrap in engine.cu);
+// the draws of all problems form one flat list of 64-draw chunks, chunk_off being its prefix sum per problem.
+struct TccResampleArgs {
+  uint32_t n_ec;
+  uint32_t nb;                          // problems in this launch
+  uint64_t first;                       // global index of problem 0
+  uint32_t B;                           // bootstraps per row
+  const uint32_t* x0;                   // B initial minstd_rand0 states (the same for every row)
+  const unsigned long long* cp_off;     // rows + 1: offsets of each row's table (indexed by global row)
+  const double* cp;                     // partial sums, the last of each row 1.0
+  const uint32_t* cp_ec;                // EC id of each table entry
+  const unsigned long long* n_draws;    // per global row: the row's total count
+  const unsigned long long* chunk_off;  // nb + 1: prefix sum of ceil(n_draws / 64) over the launch's problems
+  uint64_t n_chunks;                    // chunk_off[nb]
+  uint32_t* samp;                      // nb x n_ec output counts (zeroed by the launcher)
+};
+void launch_tcc_resample(const TccResampleArgs& a, cudaStream_t st);
 
 }  // namespace kb

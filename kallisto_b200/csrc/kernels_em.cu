@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(TPB, OCC * (TPB >= 1024 ? 1 : (TPB >= 512 ? 2 
       double nrm = 0.0;
       if (c != 0) {
         const double* al = p.alpha + (size_t)b * p.n_targets;
-        const double* mw = p.m_w + (size_t)b * p.w_stride;
+        const double* mw = p.m_w + (size_t)(p.w_set ? p.w_set[b] : b) * p.w_stride;
         double denom = 0.0;
         for (uint32_t j = e0; j < e1; ++j) {
           double a = al[p.m_tid[j]];
@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(TPB, OCC * (TPB >= 1024 ? 1 : (TPB >= 512 ? 2 
           if (st == 1 && a < zero_below) a = 0.0;
           double acc = p.single_cnt[i];                                             // :119-123
           const double* nr = p.norm + (size_t)b * p.n_multi;
-          const double* tw = p.t_w + (size_t)b * p.w_stride;
+          const double* tw = p.t_w + (size_t)(p.w_set ? p.w_set[b] : b) * p.w_stride;
           const uint32_t e0 = p.t_off[t], e1 = p.t_off[t + 1];
           for (uint32_t j = e0; j < e1; ++j)
             acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(tw[j], a), nr[p.t_midx[j]]));   // :154-156
@@ -406,6 +406,53 @@ void launch_resample(const ResampleArgs& a, cudaStream_t st) {
   const uint64_t chunks = (a.n_draws + kDrawsPerThread - 1) / kDrawsPerThread;
   dim3 grid((unsigned)((chunks + 255) / 256), (unsigned)a.nb);
   resample_kernel<<<grid, 256, 0, st>>>(a);
+}
+
+// The same draws for the (row, bootstrap) problems of quant-tcc, each over its row's sparse cumulative table.  Rows
+// hold from 0 to tens of millions of draws, so the problems are not a grid dimension: every thread takes 64-draw
+// chunks of one flat list (grid-stride) and finds its problem by binary search in the chunk prefix sum.
+__global__ void __launch_bounds__(256) tcc_resample_kernel(TccResampleArgs a) {
+  const double R = 2147483646.0;
+  const double RR = __dmul_rn(R, R);
+  for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < a.n_chunks; w += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = a.nb;                 // last problem with chunk_off[p] <= w
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (a.chunk_off[mid] <= w) lo = mid; else hi = mid;
+    }
+    const uint32_t p = lo;
+    const uint64_t g = a.first + p;
+    const uint64_t row = g / a.B;
+    const uint32_t b = (uint32_t)(g % a.B);
+    const uint64_t d0 = (w - a.chunk_off[p]) * kDrawsPerThread;
+    const uint64_t d1 = min((uint64_t)a.n_draws[row], d0 + kDrawsPerThread);
+    const uint64_t t0 = a.cp_off[row], t1 = a.cp_off[row + 1];
+    uint32_t* samp = a.samp + (size_t)p * a.n_ec;
+    uint32_t x = mulmod(a.x0[b], powmod(16807u, 2 * d0));
+    for (uint64_t d = d0; d < d1; ++d) {
+      x = mulmod(x, 16807u);
+      const double u0 = (double)(x - 1);
+      x = mulmod(x, 16807u);
+      const double u1 = (double)(x - 1);
+      double u = __ddiv_rn(__dadd_rn(u0, __dmul_rn(u1, R)), RR);
+      if (u >= 1.0) u = 0.99999999999999988897769753748;   // nextafter(1.0, 0.0)
+      // lower_bound over the row's table: its last entry is 1.0 > u, so the search ends inside the table
+      uint64_t l = t0, h = t1;
+      while (l < h) {
+        const uint64_t mid = (l + h) >> 1;
+        if (a.cp[mid] < u) l = mid + 1; else h = mid;
+      }
+      atomicAdd(&samp[a.cp_ec[l]], 1u);
+    }
+  }
+}
+
+void launch_tcc_resample(const TccResampleArgs& a, cudaStream_t st) {
+  if (a.nb == 0) return;
+  cudaMemsetAsync(a.samp, 0, (size_t)a.nb * a.n_ec * sizeof(uint32_t), st);
+  if (a.n_chunks == 0) return;
+  const unsigned g = (unsigned)std::min<uint64_t>((uint64_t)device_sm_count() * 16, (a.n_chunks + 255) / 256);
+  tcc_resample_kernel<<<g, 256, 0, st>>>(a);
 }
 
 }  // namespace kb
