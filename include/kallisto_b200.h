@@ -108,6 +108,7 @@ typedef struct kb_kernel_timings {
                                  fld, EC numbering / CSR / CSC construction, EM); CUB sort/scan launches not counted */
   double bs_resample_ms, bs_em_ms;   /* last kb_bootstrap_run: multinomial resampling, batched EM (CUDA events) */
   double pack_ms;             /* pack_kernel (+ dlist_scan_kernel with a D-list index), same launches as match_ms */
+  uint64_t em_comp_blocks;    /* last single-problem EM: blocks of the per-component kernel, 0 for the grid-wide kernel */
 } kb_kernel_timings;
 int kb_quant_enable_timing(kb_quant* q, int on);
 int kb_quant_get_timings(kb_quant* q, kb_kernel_timings* out);

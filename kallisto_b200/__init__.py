@@ -42,7 +42,8 @@ class kb_quant_opts(C.Structure):
 class kb_kernel_timings(C.Structure):
     _fields_ = [("match_ms", C.c_double), ("resolve_ms", C.c_double), ("em_ms", C.c_double), ("em_prep_ms", C.c_double),
                 ("match_launches", C.c_uint64), ("resolve_launches", C.c_uint64), ("kernel_launches", C.c_uint64),
-                ("bs_resample_ms", C.c_double), ("bs_em_ms", C.c_double), ("pack_ms", C.c_double)]
+                ("bs_resample_ms", C.c_double), ("bs_em_ms", C.c_double), ("pack_ms", C.c_double),
+                ("em_comp_blocks", C.c_uint64)]
 
 
 class kb_bus_substr(C.Structure):

@@ -399,6 +399,31 @@ void Quant::reserve_em(size_t n_ecs, size_t nnz) {
   gd(w.eff, T); gd(w.alpha, T); gd(w.norm, n1);
   if (w.emi.n < 8) w.emi.alloc(8);
   if (w.chcount.n < 2) w.chcount.alloc(2);
+  w.comp(T, (uint32_t)std::min<size_t>(n_ecs, UINT32_MAX - 1), nnz, 10000);
+}
+
+EmCompWs EmWs::comp(uint32_t T, uint32_t R, size_t nnz, int max_iter) {
+  auto g = [](auto& b, size_t need) { if (b.n < need) b.alloc(need); };
+  const size_t t1 = (size_t)T + 1, r1 = (size_t)R + 1, nz = std::max<size_t>(1, nnz);
+  const size_t slices = (size_t)device_sm_count() + 1;
+  g(c_parent, t1); g(c_rfirst, t1); g(c_iota, std::max(t1, r1)); g(c_tkey, t1); g(c_tid, t1); g(c_tloc, t1);
+  g(c_rcomp, r1); g(c_rkey, r1); g(c_rid, r1); g(c_rloc, r1); g(c_rcnt, r1); g(c_rlen, r1); g(c_roff, r1);
+  g(c_tlen, t1); g(c_toff, t1); g(c_st0, slices); g(c_sr0, slices);
+  g(c_csize, t1); g(c_cstart, t1); g(c_tsize, t1); g(c_tscan, t1); g(c_stats, 8);
+  g(c_rtid, nz); g(c_trow, nz); g(c_rw, nz); g(c_tw, nz); g(c_tsingle, t1);
+  g(c_sync, 2 * (size_t)std::max(1, max_iter));
+  g(c_tmp, emcomp_tmp_bytes(T, R));
+  EmCompWs c{};
+  c.parent = c_parent.p; c.rfirst = c_rfirst.p; c.csize = c_csize.p; c.cstart = c_cstart.p; c.iota = c_iota.p;
+  c.tkey = c_tkey.p; c.t_id = c_tid.p; c.tloc = c_tloc.p; c.tsize = c_tsize.p; c.tscan = c_tscan.p;
+  c.rcomp = c_rcomp.p; c.rkey = c_rkey.p; c.r_id = c_rid.p; c.rloc = c_rloc.p; c.r_cnt = c_rcnt.p; c.r_len = c_rlen.p;
+  c.r_off = c_roff.p; c.r_tid = c_rtid.p; c.r_w = c_rw.p; c.t_single = c_tsingle.p; c.t_len = c_tlen.p; c.t_off = c_toff.p;
+  c.t_row = c_trow.p; c.t_w = c_tw.p; c.s_t0 = c_st0.p; c.s_r0 = c_sr0.p; c.stats = c_stats.p; c.sync = c_sync.p;
+  c.sync_rounds = (int)(c_sync.n / 2);
+  c.max_slices = (int)(std::min(c_st0.n, c_sr0.n) - 1);
+  c.tmp = c_tmp.p;
+  c.tmp_bytes = c_tmp.n;
+  return c;
 }
 
 Quant::~Quant() {
@@ -1053,8 +1078,9 @@ EmResult Quant::run_em(const EcTable& ecs, const std::vector<double>& fl_trunc, 
   cudaEvent_t e0, e1;
   KB_CK(cudaEventCreate(&e0));
   KB_CK(cudaEventCreate(&e1));
+  const EmCompWs cw = emws_->comp(T, p.n_multi, h.m_tid.size(), max_iter);
   KB_CK(cudaEventRecord(e0, stream_));
-  launch_em(p, 256, stream_);
+  last_em_comp_blocks = launch_em(p, 256, stream_, &cw);
   KB_CK(cudaGetLastError());
   KB_CK(cudaEventRecord(e1, stream_));
   EmResult r;
@@ -1190,12 +1216,13 @@ EmResult Quant::run_em_device(const std::vector<double>& fl_trunc, int max_iter,
   p.rounds = w.emi.p; p.bar = w.bar.p; p.fstate = w.emi.p + 3; p.chcount = w.chcount.p;
   p.cnt_row = w.cnt_row.p; p.single_cnt = w.single_cnt.p;
   p.max_iter = max_iter; p.min_rounds = min_rounds;
+  const EmCompWs cw = w.comp(T, n_multi, nnz, max_iter);
   mark("fill launches + uploads");
   // collect_used, gather_used, ec_meta, multi_compact, row_len, ec_fill, csc_fill, stats, fill_i32, fill_f64,
   // em_gather_counts + em_kernel
   n_kernel_launches += 11 + 1;
   KB_CK(cudaEventRecord(e1, st));
-  launch_em(p, em_tpb(), st);
+  last_em_comp_blocks = launch_em(p, em_tpb(), st, &cw);
   KB_CK(cudaGetLastError());
   KB_CK(cudaEventRecord(e2, st));
   int emi[4] = {0, 0, 0, 0};

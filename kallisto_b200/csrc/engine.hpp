@@ -72,6 +72,16 @@ struct EmWs {   // grow-only device workspace of run_em_device
   DBuf<int32_t> t_single;
   DBuf<int> emi;
   DBuf<unsigned int> chcount;
+  // component layout of the single-problem EM (EmCompWs, kernels.hpp)
+  DBuf<uint32_t> c_parent, c_rfirst, c_iota, c_tkey, c_tid, c_tloc, c_rcomp, c_rkey, c_rid, c_rloc, c_rcnt, c_rlen, c_roff;
+  DBuf<uint32_t> c_tlen, c_toff, c_st0, c_sr0;
+  DBuf<unsigned long long> c_csize, c_cstart, c_tsize, c_tscan, c_stats;
+  DBuf<uint16_t> c_rtid, c_trow;
+  DBuf<double> c_rw, c_tw, c_tsingle;
+  DBuf<unsigned> c_sync;
+  DBuf<uint8_t> c_tmp;
+  // grows the buffers to T transcripts, R rows, nnz entries and max_iter rounds and hands them out
+  EmCompWs comp(uint32_t T, uint32_t R, size_t nnz, int max_iter);
 };
 
 class Index {
@@ -240,6 +250,7 @@ class Quant {
   cudaStream_t stream() const { return stream_; }
   double last_em_seconds = 0, last_prep_seconds = 0, last_bs_resample_ms = 0, last_bs_em_ms = 0;
   uint64_t n_kernel_launches = 0;   // launches of this library's own kernels by this run (CUB's are not counted)
+  int last_em_comp_blocks = 0;      // last single-problem EM: blocks of em_component_kernel, 0 for the grid-wide kernels
   // filled by run_em_device
   bool dev_stats_valid_ = false, dev_problem_valid_ = false;
   uint32_t dev_n_multi_ = 0;

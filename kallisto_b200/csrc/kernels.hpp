@@ -166,7 +166,63 @@ struct TccFill {
   double* m_w; double* t_w;             // nb x nnz
 };
 void launch_tcc_fill(const TccFill& a, cudaStream_t st);
-void launch_em(const EmProblem& p, int threads_per_block, cudaStream_t st);
+
+// Component layout of one problem (kernels_emprep.cu builds it, em_component_kernel runs on it).  The bipartite graph of
+// multi-transcript ECs and transcripts falls apart into connected components that never exchange a value; they are
+// sorted by (component, id) and cut at component boundaries into slices, one per block.  Size of a component or a
+// slice = transcripts + rows + entries.  Positions ("pos") are indices into the sorted order; every array below is
+// workspace of at least the size given (T transcripts, R multi-transcript ECs, nnz entries).
+struct EmCompWs {
+  uint32_t* parent;               // T: union-find forest, then the component (its smallest transcript id) of every transcript
+  uint32_t* rfirst;               // T: rows whose first transcript this is
+  unsigned long long* csize;      // T: size of the component rooted here
+  unsigned long long* cstart;     // T: size of all components before the one rooted here
+  uint32_t* iota;                 // max(T, R)
+  uint32_t* tkey;                 // T: component of the transcript at each pos
+  uint32_t* t_id;                 // T: pos -> transcript
+  uint32_t* tloc;                 // T: transcript -> pos inside its slice
+  unsigned long long* tsize;      // T + 1: size carried by each pos (itself, its entries, the rows it heads), then its scan
+  unsigned long long* tscan;      // T + 1
+  uint32_t* rcomp;                // R: component of each row
+  uint32_t* rkey;                 // R: component of the row at each row pos
+  uint32_t* r_id;                 // R: row pos -> row
+  uint32_t* rloc;                 // R: row -> row pos inside its slice
+  uint32_t* r_cnt;                // R: count of the row at each row pos
+  uint32_t* r_len;                // R + 1
+  uint32_t* r_off;                // R + 1: entries of the row at each row pos (CSR in slice order)
+  uint16_t* r_tid;                // nnz: slice-local transcript pos
+  double* r_w;                    // nnz
+  double* t_single;               // T: singleton count of the transcript at each pos
+  uint32_t* t_len;                // T + 1
+  uint32_t* t_off;                // T + 1: entries of the transcript at each pos (CSC in slice order)
+  uint16_t* t_row;                // nnz: slice-local row pos
+  double* t_w;                    // nnz
+  uint32_t* s_t0;                 // slices + 1: first pos of each slice
+  uint32_t* s_r0;                 // slices + 1: first row pos of each slice
+  unsigned long long* stats;      // 8: [0] total size, [1] slice target size, [2] slices, [3] largest component,
+                                  //    [4] largest slice's shared memory (bytes)
+  unsigned* sync;                 // 2 x sync_rounds: per round, blocks that changed an estimate, blocks that arrived
+  int sync_rounds;
+  int max_slices;                 // capacity of s_t0 / s_r0 minus one
+  void* tmp;
+  size_t tmp_bytes;
+};
+// Shared memory of em_component_kernel for a slice of nt transcripts and nr rows: alpha and the singleton count per
+// transcript, norm per row (doubles), then the count per row and the entry offsets of rows and transcripts (uint32).
+__host__ __device__ inline unsigned long long emcomp_smem_bytes(uint32_t nt, uint32_t nr) {
+  return 20ull * nt + 16ull * nr + 8;
+}
+size_t emcomp_tmp_bytes(uint32_t n_targets, uint32_t n_multi);
+// Largest component the component kernel takes: KB_EM_COMP_CAP (test knob, in the size units above), else unlimited.
+unsigned long long emcomp_cap();
+// Components, slices and the slice bounds; returns stats[0..4] through one device-to-host read.
+void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned long long* stats_host, cudaStream_t st);
+// Per-slice copies of counts, offsets, entries and weights with slice-local 16-bit indices.
+void emcomp_fill(const EmProblem& p, const EmCompWs& w, cudaStream_t st);
+
+// Returns the number of blocks of em_component_kernel it launched, 0 when one of the grid-wide kernels ran.
+// `cw` (optional, one problem): workspace of the component layout.
+int launch_em(const EmProblem& p, int threads_per_block, cudaStream_t st, const EmCompWs* cw = nullptr);
 
 // Device-side EM problem construction (kernels_emprep.cu)
 struct EmPrep {

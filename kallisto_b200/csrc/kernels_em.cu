@@ -237,6 +237,109 @@ __global__ void __launch_bounds__(TPB, MINB) em_single_kernel(EmProblem p) {
   }
 }
 
+// One problem whose components fit a block each (kernels.hpp, EmCompWs): every block solves one slice of whole
+// components with its alpha, norm, counts and offsets in shared memory; the entries (16-bit slice-local indices and
+// the weights) stream from the slice's contiguous part of the layout.  Pass A and pass B are em_single_kernel's, statement
+// for statement, with slice-local indices, so every row and every transcript sums exactly what it summed there.
+//
+// Components exchange no value, so there is no grid barrier.  Only the stop rule is global (EMAlgorithm.h:170-221):
+// after round i a block adds 1 to sync[2i] if it changed an estimate, then 1 to sync[2i + 1].  A block that changed
+// something knows that the global count is not zero and goes on; only a block without a change (past min_rounds) waits
+// until every block has arrived at round i and reads the count.  A block only waits for a round it has reported itself,
+// and all blocks are co-resident (cooperative launch), so no cycle of waits can form.  All blocks see a zero count in
+// the same round, so they evolve the same state and stop after the same round.
+template <int TPB>
+__global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCompWs w) {
+  extern __shared__ double s_d[];
+  __shared__ int s_zero;
+  const uint32_t b = blockIdx.x;
+  const uint32_t t0 = w.s_t0[b], nt = w.s_t0[b + 1] - t0;
+  const uint32_t r0 = w.s_r0[b], nr = w.s_r0[b + 1] - r0;
+  double* s_alpha = s_d;
+  double* s_single = s_alpha + nt;
+  double* s_norm = s_single + nt;
+  uint32_t* s_cnt = (uint32_t*)(s_norm + nr);
+  uint32_t* s_roff = s_cnt + nr;          // nr + 1
+  uint32_t* s_toff = s_roff + nr + 1;     // nt + 1
+  for (uint32_t i = threadIdx.x; i <= nt; i += TPB) {
+    s_toff[i] = w.t_off[t0 + i];
+    if (i < nt) {
+      s_alpha[i] = p.alpha[w.t_id[t0 + i]];
+      s_single[i] = w.t_single[t0 + i];
+    }
+  }
+  for (uint32_t k = threadIdx.x; k <= nr; k += TPB) {
+    s_roff[k] = w.r_off[r0 + k];
+    if (k < nr) s_cnt[k] = w.r_cnt[r0 + k];
+  }
+  __syncthreads();
+  const double zero_below = kAlphaLimit / 10.0;
+  const bool lead = b == 0 && threadIdx.x == 0;
+  int st = 0;      // 0 running, 1 final round, >= 2 finished
+  for (int it = 0;; ++it) {
+    const bool fin = st == 1;
+    // ---------------- pass A: denominators ----------------
+    for (uint32_t k = threadIdx.x; k < nr; k += TPB) {
+      const uint32_t c = s_cnt[k];
+      const uint32_t e0 = s_roff[k], e1 = s_roff[k + 1];
+      double nrm = 0.0;
+      if (c != 0) {
+        double denom = 0.0;
+#pragma unroll 4
+        for (uint32_t j = e0; j < e1; ++j) {
+          double a = s_alpha[w.r_tid[j]];
+          if (fin && a < zero_below) a = 0.0;
+          denom = __dadd_rn(denom, __dmul_rn(a, w.r_w[j]));
+        }
+        if (!(denom < kTolerance)) nrm = __ddiv_rn((double)c, denom);
+      }
+      s_norm[k] = nrm;
+    }
+    __syncthreads();
+    // ---------------- pass B: numerators, convergence test, alpha <- next ----------------
+    bool changed = false;
+    for (uint32_t i = threadIdx.x; i < nt; i += TPB) {
+      double a = s_alpha[i];
+      if (fin && a < zero_below) a = 0.0;
+      double acc = s_single[i];
+      const uint32_t e0 = s_toff[i], e1 = s_toff[i + 1];
+#pragma unroll 4
+      for (uint32_t j = e0; j < e1; ++j)
+        acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(w.t_w[j], a), s_norm[w.t_row[j]]));
+      changed = changed || (acc > kAlphaChangeLimit && (fabs(__dadd_rn(acc, -a)) / acc) > kAlphaChange);
+      s_alpha[i] = acc;
+    }
+    const bool any = __syncthreads_or(changed);
+    // ---------------- stop rule (:202-221) for the round that just ran ----------------
+    if (threadIdx.x == 0) {
+      if (any) atomicAdd(&w.sync[2 * it], 1u);
+      // release: the change count is visible before the arrival (a full fence here would stall thread 0, and with it
+      // the block's next round)
+      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(&w.sync[2 * it + 1]) : "memory");
+    }
+    if (st == 1) {
+      st = 2;
+      if (lead) p.rounds[0] = it;
+    } else if (!any && it > p.min_rounds) {
+      if (threadIdx.x == 0) {
+        while (ld_acquire_u32(&w.sync[2 * it + 1]) < gridDim.x) {}
+        s_zero = ld_acquire_u32(&w.sync[2 * it]) == 0;
+      }
+      __syncthreads();
+      if (s_zero) st = 1;
+    }
+    if (st < 2 && it + 1 == p.max_iter) {
+      if (lead) p.rounds[0] = p.max_iter;
+      st = (st == 1) ? 3 : 2;
+    }
+    if (st >= 2) {
+      if (lead) p.fstate[0] = st;
+      break;
+    }
+  }
+  for (uint32_t i = threadIdx.x; i < nt; i += TPB) p.alpha[w.t_id[t0 + i]] = s_alpha[i];
+}
+
 // Row-ordered copies of the counts the passes need: cnt_row[b][r] = counts[b][multi_ec[r]],
 // single_cnt[b][t] = counts[b][t_single[t]] (as a double) or 0.
 __global__ void em_gather_counts_kernel(EmProblem p) {
@@ -288,7 +391,42 @@ int em_max_blocks(int tpb, int nb) {
   return sms * per_sm;
 }
 
-void launch_em(const EmProblem& p, int tpb_req, cudaStream_t st) {
+namespace {
+constexpr int kCompTpb = 1024;
+
+// The component layout and em_component_kernel, when the problem's components fit: returns the blocks launched, or 0
+// (nothing launched) when a component is larger than KB_EM_COMP_CAP, a slice does not fit one block's shared memory
+// or the slices cannot all be resident at once.
+int launch_em_components(const EmProblem& p, const EmCompWs& w, cudaStream_t st) {
+  if (p.n_targets == 0 || p.max_iter < 1 || p.max_iter > w.sync_rounds) return 0;
+  const uint32_t slices = (uint32_t)std::min(device_sm_count(), w.max_slices);
+  unsigned long long s[8];
+  emcomp_cut(p, w, slices, s, st);
+  const unsigned long long n_slices = s[2], smem = s[4];
+  if (s[3] > emcomp_cap()) return 0;
+  const void* fn = (const void*)em_component_kernel<kCompTpb>;
+  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::min<unsigned long long>(smem, 1u << 30)) !=
+      cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kCompTpb, (size_t)smem) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  if ((unsigned long long)per_sm * device_sm_count() < n_slices) return 0;
+  emcomp_fill(p, w, st);
+  cudaMemsetAsync(w.sync, 0, 2 * (size_t)p.max_iter * sizeof(unsigned), st);
+  EmProblem pp = p;
+  EmCompWs ww = w;
+  void* args[] = {&pp, &ww};
+  cudaLaunchCooperativeKernel(fn, dim3((unsigned)n_slices), dim3(kCompTpb), args, (size_t)smem, st);
+  return (int)n_slices;
+}
+}  // namespace
+
+int launch_em(const EmProblem& p, int tpb_req, cudaStream_t st, const EmCompWs* cw) {
   EmProblem pp = p;
   cudaMemsetAsync(pp.bar, 0, sizeof(unsigned), st);
   {
@@ -299,13 +437,18 @@ void launch_em(const EmProblem& p, int tpb_req, cudaStream_t st) {
   void* args[] = {&pp};
   const SingleShape ss = em_single_shape();
   if (p.nb == 1 && p.w_stride == 0 && ss.fn) {
+    // an explicit KB_EM_SHAPE keeps the grid-wide kernels
+    if (cw && !getenv("KB_EM_SHAPE")) {
+      const int blocks = launch_em_components(p, *cw, st);
+      if (blocks) return blocks;
+    }
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ss.fn, ss.tpb, 0);
     int blocks = device_sm_count() * std::max(1, per_sm);
     const uint32_t work = p.n_multi > p.n_targets ? p.n_multi : p.n_targets;
     blocks = std::max(1, std::min<int>(blocks, (int)((work + ss.tpb - 1) / ss.tpb)));
     cudaLaunchCooperativeKernel(ss.fn, dim3(blocks), dim3(ss.tpb), args, 0, st);
-    return;
+    return 0;
   }
   const int tpb = tpb_req >= 1024 ? 1024 : (tpb_req >= 512 ? 512 : 256);
   const int maxb = em_max_blocks(tpb, p.nb);
@@ -315,6 +458,7 @@ void launch_em(const EmProblem& p, int tpb_req, cudaStream_t st) {
   if (const char* s = getenv("KB_EM_BLOCKS")) { const int v = atoi(s); if (v > 0) blocks = std::min(maxb, v); }   // tuning knob
   if (blocks < 1) blocks = 1;
   cudaLaunchCooperativeKernel(em_fn(tpb, em_occ()), dim3(blocks), dim3(tpb), args, (size_t)pp.nb * sizeof(int), st);
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -7,6 +7,8 @@
 // denominator pass, CSC by transcript (entries in increasing EC id) for the numerator pass of
 // em_kernel.  Sorting / scanning uses CUB device primitives (library plumbing, not a hot path:
 // ~1e6 keys once per run); the gather / weight / transpose kernels are ours.
+#include <cstdlib>
+
 #include <cub/cub.cuh>
 
 #include "kb_device.cuh"
@@ -192,6 +194,222 @@ void emprep_fill(const DevDict& dd, const EmPrep& p, uint32_t nnz, unsigned long
   }
   cudaMemsetAsync(stats2, 0, 16, st);
   stats_kernel<<<device_sm_count(), 256, 0, st>>>(p.count, p.len, p.n_ec, stats2);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Component layout of one EM problem (em_component_kernel, kernels_em.cu).  Built from the CSR / CSC of EmProblem,
+// which stay as they are (the bootstrap reuses them).
+namespace {
+
+// Roots only ever get hooked under a smaller root, so parent pointers decrease and every walk ends.  A stale read is
+// harmless: it can only show a root that has since been hooked, and the CAS on it then fails and the walk restarts.
+__device__ __forceinline__ uint32_t uf_find(const uint32_t* parent, uint32_t x) {
+  for (;;) {
+    const uint32_t q = __ldcg(parent + x);
+    if (q == x) return x;
+    x = q;
+  }
+}
+
+__global__ void comp_init_kernel(EmCompWs w, uint32_t T) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  w.parent[t] = t;
+  w.rfirst[t] = 0;
+  w.csize[t] = 0;
+}
+
+// Thread per row: every transcript of the row joins the component of the row's first transcript.
+__global__ void comp_union_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.n_multi) return;
+  const uint32_t e0 = p.m_off[r], e1 = p.m_off[r + 1];
+  if (e0 == e1) return;
+  const uint32_t t0 = p.m_tid[e0];
+  atomicAdd(&w.rfirst[t0], 1u);
+  for (uint32_t j = e0 + 1; j < e1; ++j) {
+    uint32_t a = t0, b = p.m_tid[j];
+    for (;;) {
+      a = uf_find(w.parent, a);
+      b = uf_find(w.parent, b);
+      if (a == b) break;
+      if (a < b) { const uint32_t x = a; a = b; b = x; }
+      if (atomicCAS(&w.parent[a], a, b) == a) break;
+    }
+  }
+}
+
+// After the unions: parent[t] <- root (the component's smallest transcript id).  Concurrent walks see either the old
+// parent or the root, both ancestors.
+__global__ void comp_compress_kernel(EmCompWs w, uint32_t T) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  w.parent[t] = uf_find(w.parent, t);
+  w.iota[t] = t;
+}
+
+__global__ void comp_rows_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.n_multi) return;
+  w.rcomp[r] = w.parent[p.m_tid[p.m_off[r]]];
+  w.iota[r] = r;
+}
+
+// Size carried by the transcript at each pos: itself, its entries and the rows it is the first transcript of.
+__global__ void comp_size_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > p.n_targets) return;
+  if (i == p.n_targets) { w.tsize[i] = 0; return; }      // the scan runs over T + 1 items
+  const uint32_t t = w.t_id[i];
+  const unsigned long long s = 1ull + (p.t_off[t + 1] - p.t_off[t]) + w.rfirst[t];
+  w.tsize[i] = s;
+  atomicAdd(&w.csize[w.tkey[i]], s);
+}
+
+// Component heads record where their component starts; the slice target size is ceil(total / slices), and a component
+// goes to slice floor(start / target), so there are at most `slices` slices (some may be empty).
+__global__ void comp_heads_kernel(EmProblem p, EmCompWs w, uint32_t slices) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    const unsigned long long total = w.tscan[p.n_targets];
+    const unsigned long long target = (total + slices - 1) / slices;
+    w.stats[0] = total;
+    w.stats[1] = target;
+    w.stats[2] = (total - 1) / target + 1;
+  }
+  if (i >= p.n_targets) return;
+  const uint32_t c = w.tkey[i];
+  if (i == 0 || w.tkey[i - 1] != c) {
+    w.cstart[c] = w.tscan[i];
+    atomicMax(&w.stats[3], w.csize[c]);
+  }
+}
+
+// first index of `key` (sorted by component) whose component lies in slice `s` or later
+__device__ __forceinline__ uint32_t slice_lower_bound(const uint32_t* key, uint32_t n, const unsigned long long* cstart,
+                                                      unsigned long long target, uint32_t s) {
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (cstart[key[mid]] / target < s) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Thread per slice: its first pos and row pos, and the shared memory em_component_kernel needs for it.
+__global__ void comp_bounds_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t n = (uint32_t)w.stats[2];
+  if (s >= n) return;
+  const unsigned long long target = w.stats[1];
+  const uint32_t t0 = slice_lower_bound(w.tkey, p.n_targets, w.cstart, target, s);
+  const uint32_t t1 = slice_lower_bound(w.tkey, p.n_targets, w.cstart, target, s + 1);
+  const uint32_t r0 = slice_lower_bound(w.rkey, p.n_multi, w.cstart, target, s);
+  const uint32_t r1 = slice_lower_bound(w.rkey, p.n_multi, w.cstart, target, s + 1);
+  w.s_t0[s] = t0;
+  w.s_r0[s] = r0;
+  if (s + 1 == n) { w.s_t0[n] = t1; w.s_r0[n] = r1; }
+  atomicMax(&w.stats[4], emcomp_smem_bytes(t1 - t0, r1 - r0));
+}
+
+// Slice-local positions, per-pos counts and entry counts (thread per pos and per row pos).
+__global__ void comp_local_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned long long target = w.stats[1];
+  if (i < p.n_targets) {
+    const uint32_t t = w.t_id[i];
+    w.tloc[t] = i - w.s_t0[w.cstart[w.tkey[i]] / target];
+    w.t_single[i] = p.single_cnt[t];
+    w.t_len[i] = p.t_off[t + 1] - p.t_off[t];
+  } else if (i == p.n_targets) {
+    w.t_len[i] = 0;
+  }
+  if (i < p.n_multi) {
+    const uint32_t r = w.r_id[i];
+    w.rloc[r] = i - w.s_r0[w.cstart[w.rkey[i]] / target];
+    w.r_cnt[i] = p.cnt_row[r];
+    w.r_len[i] = p.m_off[r + 1] - p.m_off[r];
+  } else if (i == p.n_multi) {
+    w.r_len[i] = 0;
+  }
+}
+
+// Entries in slice order; the order inside a row and inside a transcript's list is kept.
+__global__ void comp_entries_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.n_targets) {
+    const uint32_t t = w.t_id[i];
+    const uint32_t s0 = p.t_off[t], n = p.t_off[t + 1] - s0, d0 = w.t_off[i];
+    for (uint32_t j = 0; j < n; ++j) {
+      w.t_row[d0 + j] = (uint16_t)w.rloc[p.t_midx[s0 + j]];
+      w.t_w[d0 + j] = p.t_w[s0 + j];
+    }
+  }
+  if (i < p.n_multi) {
+    const uint32_t r = w.r_id[i];
+    const uint32_t s0 = p.m_off[r], n = p.m_off[r + 1] - s0, d0 = w.r_off[i];
+    for (uint32_t j = 0; j < n; ++j) {
+      w.r_tid[d0 + j] = (uint16_t)w.tloc[p.m_tid[s0 + j]];
+      w.r_w[d0 + j] = p.m_w[s0 + j];
+    }
+  }
+}
+
+int key_bits(uint32_t n) {
+  int bits = 1;
+  while ((1u << bits) < n && bits < 32) ++bits;
+  return bits;
+}
+
+}  // namespace
+
+size_t emcomp_tmp_bytes(uint32_t n_targets, uint32_t n_multi) {
+  const int big = (int)std::max(n_targets, n_multi) + 1;
+  size_t a = 0, b = 0, c = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+                                  (uint32_t*)nullptr, big);
+  cub::DeviceScan::ExclusiveSum(nullptr, b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, big);
+  cub::DeviceScan::ExclusiveSum(nullptr, c, (const uint32_t*)nullptr, (uint32_t*)nullptr, big);
+  return std::max(a, std::max(b, c)) + 256;
+}
+
+unsigned long long emcomp_cap() {
+  if (const char* s = getenv("KB_EM_COMP_CAP")) return strtoull(s, nullptr, 10);   // test knob
+  return ~0ull;
+}
+
+void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned long long* stats_host, cudaStream_t st) {
+  const uint32_t T = p.n_targets, R = p.n_multi;
+  const int bits = key_bits(T);
+  cudaMemsetAsync(w.stats, 0, 8 * sizeof(unsigned long long), st);
+  comp_init_kernel<<<(T + 255) / 256, 256, 0, st>>>(w, T);
+  if (R) comp_union_kernel<<<(R + 255) / 256, 256, 0, st>>>(p, w);
+  comp_compress_kernel<<<(T + 255) / 256, 256, 0, st>>>(w, T);
+  size_t tb = w.tmp_bytes;
+  cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.parent, w.tkey, w.iota, w.t_id, (int)T, 0, bits, st);
+  if (R) {
+    comp_rows_kernel<<<(R + 255) / 256, 256, 0, st>>>(p, w);
+    tb = w.tmp_bytes;
+    cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.rcomp, w.rkey, w.iota, w.r_id, (int)R, 0, bits, st);
+  }
+  comp_size_kernel<<<(T + 1 + 255) / 256, 256, 0, st>>>(p, w);
+  tb = w.tmp_bytes;
+  cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.tsize, w.tscan, (int)T + 1, st);
+  comp_heads_kernel<<<(T + 255) / 256, 256, 0, st>>>(p, w, slices);
+  comp_bounds_kernel<<<(slices + 127) / 128, 128, 0, st>>>(p, w);
+  cudaMemcpyAsync(stats_host, w.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
+  cudaStreamSynchronize(st);
+}
+
+void emcomp_fill(const EmProblem& p, const EmCompWs& w, cudaStream_t st) {
+  const uint32_t T = p.n_targets, R = p.n_multi;
+  const uint32_t n = std::max(T, R) + 1;
+  comp_local_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w);
+  size_t tb = w.tmp_bytes;
+  cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.t_len, w.t_off, (int)T + 1, st);
+  tb = w.tmp_bytes;
+  cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.r_len, w.r_off, (int)R + 1, st);
+  comp_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w);
 }
 
 }  // namespace kb

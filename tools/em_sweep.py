@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""EM kernel launch-shape sweep on the benchmark's EC table (20 x 2 M pairs): em_ms / us per round for
-KB_EM_TPB x KB_EM_BLOCKS (the library reads both at every launch).  Prints one JSON line per configuration."""
+"""EM kernel sweep on the benchmark's EC table (20 x 2 M pairs): em_ms / us per round of the default path
+(em_component_kernel) and of the launch shapes of the grid-wide kernels, KB_EM_SHAPE x KB_EM_TPB x KB_EM_BLOCKS (the
+library reads them at every launch).  Prints one JSON line per configuration."""
 import json
 import os
 import sys
@@ -29,10 +30,14 @@ def main():
         del b
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     ref = None
-    # KB_EM_SHAPE: launch shape of the single-problem kernel (-1: the batched kernel with one problem, KB_EM_TPB x KB_EM_BLOCKS)
-    for shape, name in [(-1, "em_kernel<1024,1> (batched kernel, nb = 1)"), (0, "em_single 1024 x 1"), (1, "em_single 512 x 3"),
-                        (2, "em_single 768 x 2"), (3, "em_single 1024 x 2")]:
-        os.environ["KB_EM_SHAPE"] = str(shape)
+    # KB_EM_SHAPE: launch shape of the single-problem kernel (-1: the batched kernel with one problem, KB_EM_TPB x KB_EM_BLOCKS);
+    # unset: the default path, em_component_kernel when every component fits a block
+    for shape, name in [(None, "em_component_kernel (default)"), (-1, "em_kernel<1024,1> (batched kernel, nb = 1)"),
+                        (0, "em_single 1024 x 1"), (1, "em_single 512 x 3"), (2, "em_single 768 x 2"), (3, "em_single 1024 x 2")]:
+        if shape is None:
+            os.environ.pop("KB_EM_SHAPE", None)
+        else:
+            os.environ["KB_EM_SHAPE"] = str(shape)
         os.environ["KB_EM_TPB"] = "1024"
         os.environ.pop("KB_EM_BLOCKS", None)
         os.environ["KB_EM_OCC"] = "1"
@@ -41,12 +46,12 @@ def main():
             r = mc.run_em()
             tm = mc.timings()
             if best is None or tm["em_ms"] < best[0]:
-                best = (tm["em_ms"], r["rounds"], tm["em_prep_ms"])
+                best = (tm["em_ms"], r["rounds"], tm["em_prep_ms"], tm["em_comp_blocks"])
         if ref is None:
             ref = r["est_counts"].copy()
         same = bool((r["est_counts"] == ref).all())
         print(json.dumps({"shape": shape, "kernel": name, "em_ms": best[0], "rounds": best[1], "us_per_round": best[0] * 1e3 / best[1],
-                          "prep_ms": best[2], "bit_identical_to_first": same}), flush=True)
+                          "prep_ms": best[2], "component_blocks": best[3], "bit_identical_to_first": same}), flush=True)
     mc.close()
     ix.close()
 
