@@ -211,6 +211,26 @@ int kb_tcc_bootstrap_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offset
                          const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
                          int32_t per_sample_eff, uint64_t seed, int32_t n_bootstrap, int32_t want_samples,
                          kb_tcc_bootstrap_cb cb, void* user);
+/* Gene-level output of quant-tcc (-g / -G; src/main.cpp:3026-3058, plaintext_writer_gene src/PlaintextWriter.cpp:67-112),
+ * summed on the device.  gene_of_target (n_targets) is the gene of every target, -1 for none; genes are 0 .. n_genes - 1.
+ * For every problem, tpm = counts_to_tpm(est_counts, eff_lens); every target with est_counts > 0, in increasing id, adds
+ * its est_counts to its gene's count and its tpm to its gene's TPM.  The values equal the reference's bit for bit.
+ * kb_tcc_run_genes = kb_tcc_run plus gene_counts_out and gene_tpm_out (n_samples x n_genes each, row-major).
+ * kb_tcc_bootstrap_run_genes = kb_tcc_bootstrap_run, with the bootstraps' gene counts and gene TPM (count x n_genes each,
+ * computed with the eff_lens of the problem's sample) handed to cb next to est_counts.  With n_genes == 0 both behave
+ * as kb_tcc_run / kb_tcc_bootstrap_run (gene_of_target may be NULL; cb gets NULL gene arrays). */
+int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                     const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                     int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, double* est_counts_out,
+                     int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out);
+typedef int (*kb_tcc_bootstrap_genes_cb)(void* user, uint64_t first, uint32_t count, const double* est_counts,
+                                         const int32_t* rounds, const uint32_t* samples, const double* gene_counts,
+                                         const double* gene_tpm);
+int kb_tcc_bootstrap_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids,
+                               uint32_t n_samples, const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts,
+                               const double* eff_lens, int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes,
+                               uint64_t seed, int32_t n_bootstrap, int32_t want_samples, kb_tcc_bootstrap_genes_cb cb,
+                               void* user);
 /* mean_fl_trunc -> eff_lens exactly as the reference forms them (get_frag_len_means + calc_eff_lens, src/weights.cpp:7-28,
  * 58-79): fld_mean > 0: truncated Gaussian (-l/-s); else the histogram flens[1000]; both 0/NULL: eff_len = 1 for every
  * target (quant-tcc without fragment-length information).  Host arithmetic. */

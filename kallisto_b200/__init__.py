@@ -100,12 +100,16 @@ EXPORTED_SYMBOLS = [
     "kb_quant_get_timings", "kb_quant_finalize", "kb_quant_ec_table", "kb_quant_get_flens",
     "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
     "kb_comm_unique_id", "kb_comm_create", "kb_comm_create_from_nccl", "kb_comm_create_all", "kb_comm_reserve", "kb_comm_free",
-    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
+    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
 ]
 
 # kb_tcc_bootstrap_cb: (user, first problem, count, est_counts, rounds, resampled counts or NULL) -> 0 to go on
 TCC_BOOTSTRAP_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(C.c_double), C.POINTER(C.c_int32),
                                C.POINTER(C.c_uint32))
+# kb_tcc_bootstrap_genes_cb: the same, then gene counts and gene TPM (count x n_genes) or NULL
+TCC_BOOTSTRAP_GENES_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(C.c_double),
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_uint32), C.POINTER(C.c_double),
+                                     C.POINTER(C.c_double))
 
 _lib = None
 
@@ -164,6 +168,9 @@ def lib():
     L.kb_quant_reserve.argtypes = [vp, u64, u64]
     L.kb_tcc_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, vp]
     L.kb_tcc_bootstrap_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, u64, i32, i32, TCC_BOOTSTRAP_CB, vp]
+    L.kb_tcc_run_genes.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, u32, vp, vp, vp, vp]
+    L.kb_tcc_bootstrap_run_genes.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, u32, u64, i32, i32,
+                                             TCC_BOOTSTRAP_GENES_CB, vp]
     L.kb_eff_lens.argtypes = [vp, vp, dbl, dbl, vp, C.POINTER(dbl), C.POINTER(dbl)]
     L.kb_bus_create.argtypes = [vp, C.POINTER(kb_bus_opts), C.POINTER(vp)]
     L.kb_bus_batch.argtypes = [vp, vp, vp, u32, vp, C.POINTER(u32)]
@@ -499,9 +506,20 @@ def eff_lens(index, flens=None, fld_mean=0.0, fld_sd=0.0):
     return out, m.value, s.value
 
 
-def tcc_run(index, ec_sets, rows, eff):
+def _genes_arg(index, genes):
+    """genes = (gene of every target, -1 for none; number of genes) -> (int32 array, n_genes)."""
+    gene_of, n_genes = genes
+    gene_of = np.ascontiguousarray(gene_of, np.int32)
+    if gene_of.shape != (index.num_trans,):
+        raise ValueError("genes: one gene id per target (%d), got shape %s" % (index.num_trans, gene_of.shape))
+    return gene_of, int(n_genes)
+
+
+def tcc_run(index, ec_sets, rows, eff, genes=None):
     """`kallisto quant-tcc` on the device: ec_sets = list of sorted transcript-id tuples (EC id = position), rows = per sample
-    a list of (ec id, count); eff = effective lengths (n_targets, or n_samples x n_targets) -> (est_counts (S, T), rounds (S))."""
+    a list of (ec id, count); eff = effective lengths (n_targets, or n_samples x n_targets) -> (est_counts (S, T), rounds (S)).
+    genes = (gene of every target, -1 for none; number of genes): gene-level output summed on the device
+    (kb_tcc_run_genes) -> (est_counts, rounds, gene_counts (S, G), gene_tpm (S, G))."""
     T = index.num_trans
     eo = np.zeros(len(ec_sets) + 1, np.uint64)
     tids = []
@@ -521,15 +539,24 @@ def tcc_run(index, ec_sets, rows, eff):
     per_sample = int(eff.ndim == 2)
     est = np.zeros((len(rows), T), np.float64)
     rounds = np.zeros(max(1, len(rows)), np.int32)
-    _ck(lib().kb_tcc_run(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals), _p(eff), per_sample,
-                         _p(est), _p(rounds)))
-    return est, rounds[: len(rows)]
+    if genes is None:
+        _ck(lib().kb_tcc_run(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals), _p(eff),
+                             per_sample, _p(est), _p(rounds)))
+        return est, rounds[: len(rows)]
+    gene_of, G = _genes_arg(index, genes)
+    gc = np.zeros((len(rows), max(1, G)), np.float64)
+    gt = np.zeros((len(rows), max(1, G)), np.float64)
+    _ck(lib().kb_tcc_run_genes(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals), _p(eff),
+                               per_sample, _p(gene_of), G, _p(est), _p(rounds), _p(gc), _p(gt)))
+    return est, rounds[: len(rows)], gc[:, :G], gt[:, :G]
 
 
-def tcc_bootstrap(index, ec_off, ec_tids, row_off, ec_ids, counts, eff, seed, n_bootstrap, on_chunk, want_samples=False):
+def tcc_bootstrap(index, ec_off, ec_tids, row_off, ec_ids, counts, eff, seed, n_bootstrap, on_chunk, want_samples=False,
+                  genes=None):
     """kb_tcc_bootstrap_run on CSR arrays (EC table ec_off / ec_tids, TCC rows row_off / ec_ids / counts, EC ids strictly
     increasing within a row).  on_chunk(first, est (count, T), rounds (count,), samples (count, n_ecs) or None) receives
-    the problems g = row * n_bootstrap + b in order; the arrays are copies."""
+    the problems g = row * n_bootstrap + b in order; the arrays are copies.  genes = (gene of every target, -1 for none;
+    number of genes): kb_tcc_bootstrap_run_genes, and on_chunk also receives gene_counts and gene_tpm (count, G)."""
     T = index.num_trans
     n_ecs = len(ec_off) - 1
     ec_off, ro = np.ascontiguousarray(ec_off, np.uint64), np.ascontiguousarray(row_off, np.uint64)
@@ -539,17 +566,35 @@ def tcc_bootstrap(index, ec_off, ec_tids, row_off, ec_ids, counts, eff, seed, n_
     eff = np.ascontiguousarray(eff, np.float64)
     err = []
 
+    def arrays(count, est, rounds, samples):
+        return (np.ctypeslib.as_array(est, (count, T)).copy(), np.ctypeslib.as_array(rounds, (count,)).copy(),
+                np.ctypeslib.as_array(samples, (count, n_ecs)).copy() if samples and n_ecs else None)
+
     def cb(_user, first, count, est, rounds, samples):
         try:
-            on_chunk(first, np.ctypeslib.as_array(est, (count, T)).copy(), np.ctypeslib.as_array(rounds, (count,)).copy(),
-                     np.ctypeslib.as_array(samples, (count, n_ecs)).copy() if samples and n_ecs else None)
+            on_chunk(first, *arrays(count, est, rounds, samples))
             return 0
         except BaseException as e:      # stops the run; raised again below
             err.append(e)
             return 1
-    rc = lib().kb_tcc_bootstrap_run(index._h, n_ecs, _p(ec_off), _p(ec_tids), len(ro) - 1, _p(ro), _p(ec_ids), _p(counts),
-                                    _p(eff), int(eff.ndim == 2), int(seed), int(n_bootstrap), int(want_samples),
-                                    TCC_BOOTSTRAP_CB(cb), None)
+
+    def cb_genes(_user, first, count, est, rounds, samples, gc, gt):
+        try:
+            g = [np.ctypeslib.as_array(x, (count, G)).copy() if G else np.zeros((count, 0)) for x in (gc, gt)]
+            on_chunk(first, *arrays(count, est, rounds, samples), *g)
+            return 0
+        except BaseException as e:
+            err.append(e)
+            return 1
+    if genes is None:
+        rc = lib().kb_tcc_bootstrap_run(index._h, n_ecs, _p(ec_off), _p(ec_tids), len(ro) - 1, _p(ro), _p(ec_ids),
+                                        _p(counts), _p(eff), int(eff.ndim == 2), int(seed), int(n_bootstrap),
+                                        int(want_samples), TCC_BOOTSTRAP_CB(cb), None)
+    else:
+        gene_of, G = _genes_arg(index, genes)
+        rc = lib().kb_tcc_bootstrap_run_genes(index._h, n_ecs, _p(ec_off), _p(ec_tids), len(ro) - 1, _p(ro), _p(ec_ids),
+                                              _p(counts), _p(eff), int(eff.ndim == 2), _p(gene_of), G, int(seed),
+                                              int(n_bootstrap), int(want_samples), TCC_BOOTSTRAP_GENES_CB(cb_genes), None)
     if err:
         raise err[0]
     _ck(rc)

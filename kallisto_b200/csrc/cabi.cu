@@ -386,40 +386,82 @@ int kb_quant_reserve(kb_quant* q, uint64_t n_ecs, uint64_t n_entries) {
   return guarded([&] { q->q->reserve_em(n_ecs, n_entries); });
 }
 
-int kb_tcc_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
-               const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
-               int32_t per_sample_eff, double* est_counts_out, int32_t* rounds_out) {
-  if (!ix || !ec_offsets || !row_offsets || !eff_lens || !est_counts_out || (n_ecs && !tids))
+int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                     const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                     int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, double* est_counts_out,
+                     int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out) {
+  if (!ix || !ec_offsets || !row_offsets || !eff_lens || !est_counts_out || (n_ecs && !tids) ||
+      (n_genes && (!gene_of_target || !gene_counts_out || !gene_tpm_out)))
     return fail(KB_ERR_INVALID, "kb_tcc_run: null argument");
   return guarded([&] {
     kb::TccInput in;
     in.n_ecs = n_ecs; in.ec_off = ec_offsets; in.tids = tids; in.n_samples = n_samples; in.row_off = row_offsets;
     in.ec_ids = ec_ids; in.counts = counts; in.eff_lens = eff_lens; in.per_sample_eff = per_sample_eff != 0;
-    std::vector<double> alpha;
-    const std::vector<int> rounds = kb::tcc_run(*ix->ix, in, alpha);
+    in.gene_of = gene_of_target; in.n_genes = n_genes;
+    std::vector<double> alpha, gc, gt;
+    const std::vector<int> rounds = kb::tcc_run(*ix->ix, in, alpha, &gc, &gt);
     memcpy(est_counts_out, alpha.data(), alpha.size() * sizeof(double));
+    if (n_genes) {
+      memcpy(gene_counts_out, gc.data(), gc.size() * sizeof(double));
+      memcpy(gene_tpm_out, gt.data(), gt.size() * sizeof(double));
+    }
     if (rounds_out)
       for (uint32_t i = 0; i < n_samples; ++i) rounds_out[i] = rounds[i];
   });
 }
 
-int kb_tcc_bootstrap_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
-                         const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
-                         int32_t per_sample_eff, uint64_t seed, int32_t n_bootstrap, int32_t want_samples,
-                         kb_tcc_bootstrap_cb cb, void* user) {
-  if (!ix || !ec_offsets || !row_offsets || !eff_lens || !cb || (n_ecs && !tids) || n_bootstrap < 0)
+int kb_tcc_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+               const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+               int32_t per_sample_eff, double* est_counts_out, int32_t* rounds_out) {
+  return kb_tcc_run_genes(ix, n_ecs, ec_offsets, tids, n_samples, row_offsets, ec_ids, counts, eff_lens, per_sample_eff,
+                          nullptr, 0, est_counts_out, rounds_out, nullptr, nullptr);
+}
+
+int kb_tcc_bootstrap_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids,
+                               uint32_t n_samples, const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts,
+                               const double* eff_lens, int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes,
+                               uint64_t seed, int32_t n_bootstrap, int32_t want_samples, kb_tcc_bootstrap_genes_cb cb,
+                               void* user) {
+  if (!ix || !ec_offsets || !row_offsets || !eff_lens || !cb || (n_ecs && !tids) || n_bootstrap < 0 ||
+      (n_genes && !gene_of_target))
     return fail(KB_ERR_INVALID, "kb_tcc_bootstrap_run: bad argument");
   return guarded([&] {
     kb::TccInput in;
     in.n_ecs = n_ecs; in.ec_off = ec_offsets; in.tids = tids; in.n_samples = n_samples; in.row_off = row_offsets;
     in.ec_ids = ec_ids; in.counts = counts; in.eff_lens = eff_lens; in.per_sample_eff = per_sample_eff != 0;
+    in.gene_of = gene_of_target; in.n_genes = n_genes;
     kb::tcc_bootstrap(*ix->ix, in, seed, n_bootstrap, want_samples != 0,
-                      [&](uint64_t first, uint32_t count, const double* est, const int* rounds, const uint32_t* samples) {
+                      [&](uint64_t first, uint32_t count, const double* est, const int* rounds, const uint32_t* samples,
+                          const double* gene_counts, const double* gene_tpm) {
                         static_assert(sizeof(int) == sizeof(int32_t), "rounds are handed out as int32_t");
-                        if (cb(user, first, count, est, reinterpret_cast<const int32_t*>(rounds), samples) != 0)
+                        if (cb(user, first, count, est, reinterpret_cast<const int32_t*>(rounds), samples, gene_counts,
+                               gene_tpm) != 0)
                           throw std::invalid_argument("kb_tcc_bootstrap_run: stopped by the callback");
                       });
   });
+}
+
+namespace {
+struct TccBootstrapCbAdapter {     // kb_tcc_bootstrap_cb behind a kb_tcc_bootstrap_genes_cb that ignores the genes
+  kb_tcc_bootstrap_cb cb;
+  void* user;
+  static int call(void* self, uint64_t first, uint32_t count, const double* est, const int32_t* rounds,
+                  const uint32_t* samples, const double*, const double*) {
+    const auto* a = static_cast<const TccBootstrapCbAdapter*>(self);
+    return a->cb(a->user, first, count, est, rounds, samples);
+  }
+};
+}  // namespace
+
+int kb_tcc_bootstrap_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                         const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                         int32_t per_sample_eff, uint64_t seed, int32_t n_bootstrap, int32_t want_samples,
+                         kb_tcc_bootstrap_cb cb, void* user) {
+  if (!cb) return fail(KB_ERR_INVALID, "kb_tcc_bootstrap_run: bad argument");
+  TccBootstrapCbAdapter a{cb, user};
+  return kb_tcc_bootstrap_run_genes(ix, n_ecs, ec_offsets, tids, n_samples, row_offsets, ec_ids, counts, eff_lens,
+                                    per_sample_eff, nullptr, 0, seed, n_bootstrap, want_samples, &TccBootstrapCbAdapter::call,
+                                    &a);
 }
 
 int kb_eff_lens(const kb_index* ix, const uint32_t* flens, double fld_mean, double fld_sd, double* eff_out, double* mean_out,

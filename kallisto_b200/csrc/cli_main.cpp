@@ -24,12 +24,18 @@
 #include <sstream>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
+
+#include <zlib.h>
 
 #include "../../include/kallisto_b200.h"
 // Bound weakly: the command line also links against stand-ins of the library that carry only the entry points of the
-// host pipeline (tests/stub); there `quant-tcc -b` reports the missing entry point instead of failing to link.
+// host pipeline (tests/stub); there `quant-tcc -b` and `quant-tcc -g / -G` report the missing entry point instead of
+// failing to link.
 #pragma weak kb_tcc_bootstrap_run
+#pragma weak kb_tcc_run_genes
+#pragma weak kb_tcc_bootstrap_run_genes
 #include "fastx.hpp"
 #include "h5_reader.hpp"
 #include "h5_writer.hpp"
@@ -1386,8 +1392,9 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
 // abundances from pre-computed transcript-compatibility counts.  Every row of the TCC matrix is one EM over the
 // equivalence classes of the EC file; all rows are solved on the device by the batched EM kernel (kb_tcc_run), and
 // their bootstraps (-b) likewise, every (row, bootstrap) pair its own problem (kb_tcc_bootstrap_run).
-// Supported: -i, -e (required here), -o, -l/-s, -f, -t, -b, -d/--seed, --matrix-to-files, --matrix-to-directories,
-// --plaintext.  Gene-level output (-g/-G), priors, --long, -T and a per-sample abundance.h5 are refused loudly.
+// Supported: -i, -e (required here), -o, -l/-s, -f, -t, -b, -d/--seed, -g/--genemap, -G/--gtf, --matrix-to-files,
+// --matrix-to-directories, --plaintext.  Gene-level output is summed on the device (kb_tcc_run_genes,
+// kb_tcc_bootstrap_run_genes).  Priors, --long, -T and a per-sample abundance.h5 are refused loudly.
 // Deliberate differences from the reference:
 //   - -b on a matrix file without --matrix-to-files / --matrix-to-directories, or without --plaintext, is refused: the
 //     reference (built without HDF5) runs and silently writes no bootstraps there.
@@ -1410,6 +1417,10 @@ void usage_tcc() {
             << "-b, --bootstrap-samples=INT   Number of bootstrap samples (default: 0); with a matrix file only" << endl
             << "                              together with --matrix-to-files or --matrix-to-directories and --plaintext" << endl
             << "    --seed=INT                Seed for the bootstrap sampling (default: 42)" << endl
+            << "-g, --genemap                 File for mapping transcripts to genes" << endl
+            << "                              (required for obtaining gene-level abundances)" << endl
+            << "-G, --gtf=FILE                GTF file for transcriptome information" << endl
+            << "                              (can be used instead of --genemap for obtaining gene-level abundances)" << endl
             << "    --matrix-to-files         Reorganize matrix output into abundance tsv files" << endl
             << "    --matrix-to-directories   Reorganize matrix output into abundance tsv files across" << endl
             << "                              multiple directories" << endl
@@ -1434,6 +1445,202 @@ void write_sparse_matrix(const std::string& path, const std::vector<std::vector<
       }
   std::ofstream of(path, std::ios::out | std::ios::binary);
   of.write(out.data(), (std::streamsize)out.size());
+}
+
+// The gene model of quant-tcc's gene-level output (Transcriptome, src/GeneModel.cpp), reduced to what that output reads:
+// the genes in id order with their common names, and the gene of every target (-1: none, left out of every sum).
+struct GeneModel {
+  std::vector<std::string> name, common;
+  std::vector<int32_t> gene_of;
+};
+
+std::unordered_map<std::string, int32_t> target_ids(const std::vector<std::string>& targets) {
+  std::unordered_map<std::string, int32_t> m;
+  for (size_t i = 0; i < targets.size(); ++i) m.insert({targets[i], (int32_t)i});
+  return m;
+}
+
+// Transcriptome::parseGeneMap (src/GeneModel.cpp:580-632): every non-empty line is `transcript gene [common name]`
+// (further columns ignored); genes are numbered in order of first appearance, and a later line for a transcript
+// reassigns it.  Prints the reference's message and returns false on an error.
+bool parse_genemap(const std::string& fn, const std::vector<std::string>& targets, GeneModel& gm) {
+  const auto tr = target_ids(targets);
+  std::unordered_map<std::string, int32_t> gid;
+  gm.gene_of.assign(targets.size(), -1);
+  std::ifstream in(fn);
+  if (!in.is_open()) { cerr << "Error: could not open file " << fn << endl; return false; }
+  std::string line;
+  while (getline(in, line)) {
+    if (line.empty()) continue;
+    std::stringstream ss(line);
+    std::string txp, gene, common;
+    ss >> txp >> gene >> common;
+    if (gene.empty()) { cerr << "Error: No gene associated with transcript " << txp << " in " << fn << endl; return false; }
+    const auto it = tr.find(txp);
+    if (it == tr.end()) { cerr << "Error: Invalid transcript: " << txp << " in " << fn << endl; return false; }
+    auto g = gid.find(gene);
+    if (g == gid.end()) {
+      g = gid.insert({gene, (int32_t)gm.name.size()}).first;
+      gm.name.push_back(gene);
+      gm.common.push_back(common);
+    }
+    gm.gene_of[it->second] = g->second;
+  }
+  return true;
+}
+
+// Transcriptome::parseGTF / addGTFLine (src/GeneModel.cpp:268-578) with every chromosome accepted, as quant-tcc calls it;
+// plain or gzip (zlib's gzread, like the reference).  Only `gene` and `transcript` lines carry what gene-level output
+// reads.  Their quirks are kept:
+//   - a `gene` line appends ".<gene_version>" to a gene_id without a '.'; a duplicate gene adds a second entry to the
+//     gene list, but its name keeps the id of the first;
+//   - a `transcript` line looks its transcript up with ".<transcript_version>" (when the id has no '.') and then bare,
+//     and its gene with ".<gene_version>" appended whether or not the id has a '.' (src/GeneModel.cpp:450 tests the
+//     empty gene model of the line), then bare; a gene that has had no `gene` line yet gives -1;
+//   - the first `transcript` line of a target decides its gene;
+//   - attributes are read until a `gene` line's third counted key is gene_id, or a `transcript` line has counted four of
+//     gene_id, gene_version, transcript_id, transcript_version.
+bool parse_gtf(const std::string& fn, const std::vector<std::string>& targets, GeneModel& gm) {
+  const auto tr = target_ids(targets);
+  std::unordered_map<std::string, int32_t> gid;
+  std::vector<char> seen(targets.size(), 0);
+  gm.gene_of.assign(targets.size(), -1);
+  std::string text;
+  {
+    gzFile f = gzopen(fn.c_str(), "r");
+    if (!f) { cerr << "Error: could not open file " << fn << endl; return false; }
+    char buf[1 << 16];
+    int n;
+    while ((n = gzread(f, buf, sizeof(buf))) > 0) text.append(buf, (size_t)n);
+    const bool bad = n < 0;
+    gzclose(f);
+    if (bad) { cerr << "Error: could not read file " << fn << endl; return false; }
+  }
+  size_t missing = 0;
+  const size_t npos = std::string::npos;
+  for (size_t a = 0; a < text.size();) {
+    size_t e = text.find('\n', a);
+    if (e == npos) e = text.size();
+    const std::string line = text.substr(a, e - a);
+    a = e + 1;
+    if (line.empty() || line[0] == '#') continue;
+    const size_t t1 = line.find('\t'), t2 = t1 == npos ? npos : line.find('\t', t1 + 1);
+    if (t2 == npos) continue;
+    size_t t = line.find('\t', t2 + 1);
+    const std::string type = line.substr(t2 + 1, t == npos ? npos : t - t2 - 1);
+    const bool is_gene = type == "gene";
+    if (!is_gene && type != "transcript") continue;
+    for (int i = 0; i < 5 && t != npos; ++i) t = line.find('\t', t + 1);    // start, stop, score, strand, phase
+    if (t == npos) { cerr << "Error: malformed GTF line in " << fn << ": " << line << endl; return false; }
+    std::string gene, gversion, txp, tversion, common;
+    int keycount = 0;
+    for (size_t p = t + 1; p != npos;) {
+      const size_t q = line.find('"', p);
+      if (q == npos) break;
+      const size_t s = line.find('"', q + 1);
+      if (s == npos) break;
+      const std::string key = line.substr(p, q - p - 1), value = line.substr(q + 1, s - q - 1);
+      if (key == "gene_id") { ++keycount; gene = value; }
+      else if (key == "gene_version") { ++keycount; gversion = value; }
+      if (is_gene) {
+        if (key == "gene_name") { ++keycount; common = value; }
+        else if (key == "gene_id" && keycount == 3) break;
+      } else {
+        if (key == "transcript_id") { ++keycount; txp = value; }
+        else if (key == "transcript_version") { ++keycount; tversion = value; }
+        if (keycount == 4) break;
+      }
+      if ((p = line.find(' ', s)) != npos && ++p >= line.size()) break;
+    }
+    if (is_gene) {
+      if (!gversion.empty() && gene.find('.') == npos) gene += "." + gversion;
+      gid.insert({gene, (int32_t)gm.name.size()});
+      gm.name.push_back(gene);
+      gm.common.push_back(common);
+      continue;
+    }
+    auto it = tr.end();
+    if (!tversion.empty() && txp.find('.') == npos) it = tr.find(txp + "." + tversion);
+    if (it == tr.end()) it = tr.find(txp);
+    if (it == tr.end()) { ++missing; continue; }
+    auto g = gid.end();
+    if (!gversion.empty()) g = gid.find(gene + "." + gversion);
+    if (g == gid.end()) g = gid.find(gene);
+    if (!seen[it->second]) {
+      seen[it->second] = 1;
+      gm.gene_of[it->second] = g == gid.end() ? -1 : g->second;
+    }
+  }
+  if (missing) cerr << "Warning: " << missing << " transcripts were defined in GTF file, but not in the index" << endl;
+  return true;
+}
+
+// plaintext_writer_gene (src/PlaintextWriter.cpp:67-112): every gene, zero or not
+void write_gene_abundance(const std::string& path, const GeneModel& gm, const double* gc, const double* gt) {
+  std::ofstream of(path, std::ios::out | std::ios::binary);
+  if (!of.is_open()) {
+    cerr << "Error: Couldn't open file: " << path << endl;
+    exit(1);
+  }
+  std::string out = "gene_id\tgene_name\test_counts\ttpm\n";
+  for (size_t g = 0; g < gm.name.size(); ++g) {
+    out += gm.name[g];
+    out += '\t';
+    out += gm.common[g];
+    out += '\t';
+    append_double(out, gc[g]);
+    out += '\t';
+    append_double(out, gt[g]);
+    out += '\n';
+  }
+  of.write(out.data(), (std::streamsize)out.size());
+}
+
+// The bootstrap files of quant-tcc, written chunk by chunk as the device hands the (row, bootstrap) problems over
+struct TccBsCtx {
+  const std::string* output;
+  bool is_matrix, dirs, per_sample;
+  int B, threads;
+  uint32_t T;
+  const std::vector<std::string>* names;
+  const std::vector<uint32_t>* lens;
+  const std::vector<double>* eff;
+  const std::vector<double>* est;
+  const std::vector<char>* empty_row;
+  const GeneModel* genes;                 // gene files next to every matrix row's bootstrap file, or nullptr
+  const std::vector<double>* gene_counts; // the rows' own gene sums (an empty row's bootstraps are copies of them)
+  const std::vector<double>* gene_tpm;
+};
+
+int write_tcc_bs_chunk(void* user, uint64_t first, uint32_t count, const double* bs_est, const int32_t*, const uint32_t*,
+                       const double* bs_gc, const double* bs_gt) {
+  const TccBsCtx& c = *static_cast<const TccBsCtx*>(user);
+  const size_t G = c.genes ? c.genes->name.size() : 0;
+  auto write_one = [&](uint32_t i) {
+    const uint64_t g = first + i, r = g / c.B, b = g % c.B;
+    std::string path, gpath;
+    if (!c.is_matrix) path = *c.output + "/bs_abundance_" + std::to_string(b) + ".tsv";
+    else if (c.dirs) {
+      path = *c.output + "/abundance_" + std::to_string(r + 1) + "/bs_abundance_" + std::to_string(b) + ".tsv";
+      gpath = *c.output + "/abundance_" + std::to_string(r + 1) + "/bs_abundance.gene_" + std::to_string(b) + ".tsv";
+    } else {
+      path = *c.output + "/bs_abundance_" + std::to_string(r + 1) + "_" + std::to_string(b) + ".tsv";
+      gpath = *c.output + "/bs_abundance.gene_" + std::to_string(r + 1) + "_" + std::to_string(b) + ".tsv";
+    }
+    const bool empty = (*c.empty_row)[r];
+    const double* a = empty ? c.est->data() + r * c.T : bs_est + (size_t)i * c.T;
+    write_abundance(path, *c.names, *c.lens, c.eff->data() + (c.per_sample ? r : 0) * (size_t)c.T, a);
+    if (c.genes && c.is_matrix)
+      write_gene_abundance(gpath, *c.genes, empty ? c.gene_counts->data() + r * G : bs_gc + (size_t)i * G,
+                           empty ? c.gene_tpm->data() + r * G : bs_gt + (size_t)i * G);
+  };
+  const uint32_t nt = (uint32_t)std::min<int64_t>(c.threads, count);
+  std::vector<std::thread> pool;
+  for (uint32_t t = 1; t < nt; ++t)
+    pool.emplace_back([&, t] { for (uint32_t i = t; i < count; i += nt) write_one(i); });
+  for (uint32_t i = 0; i < count; i += nt) write_one(i);
+  for (auto& th : pool) th.join();
+  return 0;
 }
 
 int cmd_quant_tcc(int argc, char** argv) {
@@ -1501,7 +1708,9 @@ int cmd_quant_tcc(int argc, char** argv) {
   if (ecfile.empty()) { cerr << ERROR_STR << " equivalence class file must be supplied (-e)" << endl; ret = false; }
   else if (stat(ecfile.c_str(), &stt) != 0) { cerr << ERROR_STR << " equivalence class file not found " << ecfile << endl; ret = false; }
   if (!fldfile.empty() && stat(fldfile.c_str(), &stt) != 0) { cerr << ERROR_STR << " fragment length distribution file not found " << fldfile << endl; ret = false; }
-  if (!genemap.empty() || !gtf.empty()) { cerr << ERROR_STR << " gene-level output (--genemap / --gtf) is not supported by this build" << endl; ret = false; }
+  if (!genemap.empty() && !gtf.empty()) { cerr << ERROR_STR << " Cannot supply both --genemap and --gtf" << endl; ret = false; }
+  if (!gtf.empty() && stat(gtf.c_str(), &stt) != 0) { cerr << ERROR_STR << " GTF file not found " << gtf << endl; ret = false; }
+  if (!genemap.empty() && stat(genemap.c_str(), &stt) != 0) { cerr << ERROR_STR << " file for mapping transcripts to genes not found " << genemap << endl; ret = false; }
   if (!priors.empty() || long_flag || !txnames.empty()) { cerr << ERROR_STR << " --priors, --long and --txnames are not supported by this build" << endl; ret = false; }
   if (bootstrap > 0 && (!matrix_to_files || !plaintext) && !tccfile.empty()) {
     std::ifstream in(tccfile);
@@ -1677,18 +1886,32 @@ int cmd_quant_tcc(int argc, char** argv) {
     if (per_sample) fld_mat[r] = {m, s};
     else for (auto& x : fld_mat) x = {m, s};
   }
-  cerr << "[quant] Running EM algorithm..." << endl;
-  std::vector<double> est(nrow * (size_t)T);
-  std::vector<int32_t> rounds(nrow + 1);
-  KB_TRY(kb_tcc_run(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow, row_off.data(),
-                    ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(), eff.data(), per_sample ? 1 : 0,
-                    est.data(), rounds.data()));
-  cerr << " done" << endl << endl;
-  // ---- outputs (src/main.cpp:2928-2946, 3040-3215)
   std::vector<std::string> names(T);
   std::vector<uint32_t> lens(T);
   for (uint32_t i = 0; i < T; ++i) names[i] = kb_index_target_name(ix, i);
   kb_index_target_lens(ix, lens.data());
+  // ---- gene model (src/main.cpp:2975-2980)
+  const bool gene_level = !genemap.empty() || !gtf.empty();
+  GeneModel gm;
+  if (!genemap.empty() && !parse_genemap(genemap, names, gm)) return 1;
+  if (!gtf.empty() && !parse_gtf(gtf, names, gm)) return 1;
+  const uint32_t G = (uint32_t)gm.name.size();
+  cerr << "[quant] Running EM algorithm..." << endl;
+  std::vector<double> est(nrow * (size_t)T), gene_counts(gene_level ? nrow * (size_t)G : 0), gene_tpm(gene_counts.size());
+  std::vector<int32_t> rounds(nrow + 1);
+  if (gene_level) {
+    if (!kb_tcc_run_genes) { cerr << "Error: this libkallisto_b200 has no kb_tcc_run_genes" << endl; return 1; }
+    KB_TRY(kb_tcc_run_genes(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow,
+                            row_off.data(), ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(),
+                            eff.data(), per_sample ? 1 : 0, gm.gene_of.data(), G, est.data(), rounds.data(),
+                            gene_counts.data(), gene_tpm.data()));
+  } else {
+    KB_TRY(kb_tcc_run(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow, row_off.data(),
+                      ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(), eff.data(), per_sample ? 1 : 0,
+                      est.data(), rounds.data()));
+  }
+  cerr << " done" << endl << endl;
+  // ---- outputs (src/main.cpp:2928-2946, 3040-3215)
   {
     std::string out;
     for (uint32_t i = 0; i < T; ++i) { out += names[i]; out += "\n"; }
@@ -1696,11 +1919,13 @@ int cmd_quant_tcc(int argc, char** argv) {
     of.write(out.data(), (std::streamsize)out.size());
   }
   if (is_matrix) {
-    std::vector<std::vector<std::pair<int, double>>> ab(nrow), tpm_m(nrow), el(nrow);
+    std::vector<std::vector<std::pair<int, double>>> ab(nrow), tpm_m(nrow), el(nrow), ab_g(nrow), tpm_g(nrow);
     std::vector<double> tpm(T);
     for (size_t r = 0; r < nrow; ++r) {
       const double* a = est.data() + r * T;
       const double* e = eff.data() + (per_sample ? r : 0) * (size_t)T;
+      const double* gc = gene_counts.data() + r * G;
+      const double* gt = gene_tpm.data() + r * G;
       kb_counts_to_tpm(a, e, T, tpm.data());
       for (uint32_t i = 0; i < T; ++i)
         if (a[i] > 0.0) {
@@ -1708,6 +1933,12 @@ int cmd_quant_tcc(int argc, char** argv) {
           tpm_m[r].push_back({(int)i, tpm[i]});
           if (calc_eff) el[r].push_back({(int)i, e[i]});
         }
+      if (gene_level)
+        for (uint32_t g = 0; g < G; ++g)
+          if (gc[g] > 0.0) {
+            ab_g[r].push_back({(int)g, gc[g]});
+            tpm_g[r].push_back({(int)g, gt[g]});
+          }
       if (matrix_to_dirs) {
         const std::string dir = output + "/abundance_" + std::to_string(r + 1);     // src/main.cpp:3063-3084
         struct stat ds;
@@ -1718,60 +1949,58 @@ int cmd_quant_tcc(int argc, char** argv) {
           return 1;
         }
         write_abundance(dir + "/abundance.tsv", names, lens, e, a);
+        if (gene_level) write_gene_abundance(dir + "/abundance.gene.tsv", gm, gc, gt);
       } else if (matrix_to_files) {
         write_abundance(output + "/abundance_" + std::to_string(r + 1) + ".tsv", names, lens, e, a);
+        if (gene_level) write_gene_abundance(output + "/abundance.gene_" + std::to_string(r + 1) + ".tsv", gm, gc, gt);
       }
     }
     write_sparse_matrix(output + "/matrix.abundance.mtx", ab, T);
     write_sparse_matrix(output + "/matrix.abundance.tpm.mtx", tpm_m, T);
     if (calc_eff) write_sparse_matrix(output + "/matrix.efflens.mtx", el, T);
+    if (gene_level) {
+      write_sparse_matrix(output + "/matrix.abundance.gene.mtx", ab_g, G);
+      write_sparse_matrix(output + "/matrix.abundance.gene.tpm.mtx", tpm_g, G);
+      std::string out;                                              // writeGeneList(..., true), src/PlaintextWriter.cpp:300-315
+      for (auto& n : gm.name) { out += n; out += "\n"; }
+      std::ofstream of(output + "/genes.txt", std::ios::binary);
+      of.write(out.data(), (std::streamsize)out.size());
+    }
   } else {
     write_abundance(output + "/abundance.tsv", names, lens, eff.data(), est.data());
+    if (gene_level) write_gene_abundance(output + "/abundance.gene.tsv", gm, gene_counts.data(), gene_tpm.data());
   }
   if (bootstrap > 0) {
     // src/main.cpp:3109-3178: bs_abundance_<b>.tsv (non-matrix file), bs_abundance_<row>_<b>.tsv (--matrix-to-files) or
     // abundance_<row>/bs_abundance_<b>.tsv (--matrix-to-directories), rows numbered from 1, each written with its row's
     // eff_lens.  A matrix row without any non-zero estimate gets B copies of that (zero) estimate.  The device hands the
-    // (row, bootstrap) problems over chunk by chunk; up to -t threads write a chunk's files.
+    // (row, bootstrap) problems over chunk by chunk; up to -t threads write a chunk's files.  With genes, a matrix row's
+    // bootstraps also get bs_abundance.gene_<row>_<b>.tsv or abundance_<row>/bs_abundance.gene_<b>.tsv, summed on the
+    // device; a non-matrix file gets no gene bootstrap files, as in the reference.
     cerr << "[bstrp] running EM for " << pretty_num((size_t)nrow * bootstrap) << " bootstraps" << endl;
     std::vector<char> empty_row(nrow, 0);
     if (is_matrix)
       for (size_t r = 0; r < nrow; ++r)
         empty_row[r] = std::none_of(est.begin() + r * T, est.begin() + (r + 1) * T, [](double x) { return x > 0.0; });
-    struct Ctx {
-      const std::string* output;
-      bool is_matrix, dirs, per_sample;
-      int B, threads;
-      uint32_t T;
-      const std::vector<std::string>* names;
-      const std::vector<uint32_t>* lens;
-      const std::vector<double>* eff;
-      const std::vector<double>* est;
-      const std::vector<char>* empty_row;
-    } ctx{&output, is_matrix, matrix_to_dirs != 0, per_sample, bootstrap, threads, T, &names, &lens, &eff, &est, &empty_row};
-    auto write_chunk = [](void* user, uint64_t first, uint32_t count, const double* bs_est, const int32_t*, const uint32_t*) -> int {
-      const Ctx& c = *static_cast<const Ctx*>(user);
-      auto write_one = [&](uint32_t i) {
-        const uint64_t g = first + i, r = g / c.B, b = g % c.B;
-        std::string path;
-        if (!c.is_matrix) path = *c.output + "/bs_abundance_" + std::to_string(b) + ".tsv";
-        else if (c.dirs) path = *c.output + "/abundance_" + std::to_string(r + 1) + "/bs_abundance_" + std::to_string(b) + ".tsv";
-        else path = *c.output + "/bs_abundance_" + std::to_string(r + 1) + "_" + std::to_string(b) + ".tsv";
-        const double* a = (*c.empty_row)[r] ? c.est->data() + r * c.T : bs_est + (size_t)i * c.T;
-        write_abundance(path, *c.names, *c.lens, c.eff->data() + (c.per_sample ? r : 0) * (size_t)c.T, a);
+    const bool bs_genes = gene_level && is_matrix;
+    TccBsCtx ctx{&output, is_matrix, matrix_to_dirs != 0, per_sample, bootstrap, threads, T, &names, &lens, &eff, &est,
+                 &empty_row, bs_genes ? &gm : nullptr, &gene_counts, &gene_tpm};
+    if (bs_genes) {
+      if (!kb_tcc_bootstrap_run_genes) { cerr << "Error: this libkallisto_b200 has no kb_tcc_bootstrap_run_genes" << endl; return 1; }
+      KB_TRY(kb_tcc_bootstrap_run_genes(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow,
+                                        row_off.data(), ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(),
+                                        eff.data(), per_sample ? 1 : 0, gm.gene_of.data(), G, (uint64_t)seed, bootstrap, 0,
+                                        write_tcc_bs_chunk, &ctx));
+    } else {
+      auto write_chunk = [](void* user, uint64_t first, uint32_t count, const double* bs_est, const int32_t* rounds,
+                            const uint32_t* samples) -> int {
+        return write_tcc_bs_chunk(user, first, count, bs_est, rounds, samples, nullptr, nullptr);
       };
-      const uint32_t nt = (uint32_t)std::min<int64_t>(c.threads, count);
-      std::vector<std::thread> pool;
-      for (uint32_t t = 1; t < nt; ++t)
-        pool.emplace_back([&, t] { for (uint32_t i = t; i < count; i += nt) write_one(i); });
-      for (uint32_t i = 0; i < count; i += nt) write_one(i);
-      for (auto& th : pool) th.join();
-      return 0;
-    };
-    if (!kb_tcc_bootstrap_run) { cerr << "Error: this libkallisto_b200 has no kb_tcc_bootstrap_run" << endl; return 1; }
-    KB_TRY(kb_tcc_bootstrap_run(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow, row_off.data(),
-                                ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(), eff.data(),
-                                per_sample ? 1 : 0, (uint64_t)seed, bootstrap, 0, write_chunk, &ctx));
+      if (!kb_tcc_bootstrap_run) { cerr << "Error: this libkallisto_b200 has no kb_tcc_bootstrap_run" << endl; return 1; }
+      KB_TRY(kb_tcc_bootstrap_run(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow, row_off.data(),
+                                  ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(), eff.data(),
+                                  per_sample ? 1 : 0, (uint64_t)seed, bootstrap, 0, write_chunk, &ctx));
+    }
     cerr << " done" << endl << endl;
   }
   if (calc_eff) {

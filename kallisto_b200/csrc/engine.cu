@@ -1573,12 +1573,58 @@ struct TccShape {
     return p;
   }
 };
+
+// Gene-level output: gene -> member transcripts (CSR, increasing id) from in.gene_of, and the gene sums of up to `nb_max`
+// problems at a time.  Without genes (in.n_genes == 0) nothing is allocated and run() does nothing.
+struct TccGenes {
+  uint32_t G = 0;
+  DBuf<uint32_t> g_off, g_tid;
+  DBuf<double> total, counts, tpm;
+
+  TccGenes(uint32_t T, const TccInput& in, uint64_t nb_max, cudaStream_t st) : G(in.n_genes) {
+    if (!G) return;
+    if (!in.gene_of) throw Error("kallisto_b200: n_genes > 0 without a gene of every target");
+    std::vector<uint32_t> off(G + 1, 0), tid;
+    for (uint32_t t = 0; t < T; ++t) {
+      const int32_t g = in.gene_of[t];
+      if (g < -1 || (g >= 0 && (uint32_t)g >= G)) throw Error("kallisto_b200: a target's gene id is out of range");
+      if (g >= 0) ++off[g + 1];
+    }
+    for (uint32_t g = 0; g < G; ++g) off[g + 1] += off[g];
+    tid.resize(off[G]);
+    {
+      std::vector<uint32_t> fill(off.begin(), off.end() - 1);
+      for (uint32_t t = 0; t < T; ++t)
+        if (in.gene_of[t] >= 0) tid[fill[in.gene_of[t]]++] = t;
+    }
+    g_off.alloc(G + 1); g_off.upload(off.data(), G + 1, st);
+    g_tid.alloc(std::max<size_t>(1, tid.size())); g_tid.upload(tid.data(), tid.size(), st);
+    total.alloc(nb_max); counts.alloc(nb_max * G); tpm.alloc(nb_max * G);
+    KB_CK(cudaStreamSynchronize(st));     // the host vectors go out of scope
+  }
+  // bytes per problem, for the sizing of chunks
+  static size_t per_problem(const TccInput& in) { return in.n_genes ? (size_t)in.n_genes * 16 + 8 : 0; }
+  // the gene sums of nb problems whose estimates are in alpha (their final states in fstate), into counts / tpm
+  void run(uint32_t nb, uint32_t T, const double* alpha, const int* fstate, const double* eff, uint64_t eff_stride,
+           const uint32_t* w_set, cudaStream_t st) {
+    if (!G) return;
+    TccGeneArgs a{};
+    a.nb = nb; a.n_targets = T; a.n_genes = G; a.alpha = alpha; a.fstate = fstate;
+    a.eff = eff; a.eff_stride = eff_stride; a.w_set = w_set; a.g_off = g_off.p; a.g_tid = g_tid.p;
+    a.total = total.p; a.gene_counts = counts.p; a.gene_tpm = tpm.p;
+    launch_tcc_genes(a, st);
+    KB_CK(cudaGetLastError());
+  }
+};
 }  // namespace
 
-std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out) {
+std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out, std::vector<double>* gene_counts_out,
+                         std::vector<double>* gene_tpm_out) {
   KB_CK(cudaSetDevice(ix.device));
-  const uint32_t T = ix.flat.num_targets(), nE = in.n_ecs, S = in.n_samples;
+  const uint32_t T = ix.flat.num_targets(), nE = in.n_ecs, S = in.n_samples, G = in.n_genes;
   alpha_out.assign((size_t)S * T, 0.0);
+  if (G && (!gene_counts_out || !gene_tpm_out)) throw Error("kallisto_b200: gene-level output without its buffers");
+  if (G) { gene_counts_out->assign((size_t)S * G, 0.0); gene_tpm_out->assign((size_t)S * G, 0.0); }
   std::vector<int> rounds(S, 0);
   if (S == 0) return rounds;
   StreamGuard sg;
@@ -1593,10 +1639,11 @@ std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alp
   DBuf<int> d_emi;
   DBuf<unsigned> d_ch, d_bar;
   // samples per chunk: weights dominate (16 bytes per entry and sample); ~2 GB of work space
-  const size_t per = (size_t)nnz * 16 + (size_t)nE * 4 + ((size_t)T + n_multi) * 8;
+  const size_t per = (size_t)nnz * 16 + (size_t)nE * 4 + ((size_t)T + n_multi) * 8 + TccGenes::per_problem(in);
   int chunk = (int)std::max<size_t>(1, std::min<size_t>(S, ((size_t)2 << 30) / std::max<size_t>(1, per)));
   if (const char* s = getenv("KB_TCC_CHUNK")) { const int v = atoi(s); if (v > 0) chunk = std::min<int>((int)S, v); }   // tests
   chunk = std::min(chunk, KB_EM_MAX_BATCH);
+  TccGenes genes(T, in, (uint64_t)chunk, st);
   d_counts.alloc((size_t)chunk * std::max<uint32_t>(1, nE));
   d_mw.alloc(std::max<size_t>(1, (size_t)chunk * nnz)); d_tw.alloc(std::max<size_t>(1, (size_t)chunk * nnz));
   d_alpha.alloc((size_t)chunk * T); d_norm.alloc(std::max<size_t>(1, (size_t)chunk * n_multi));
@@ -1624,8 +1671,13 @@ std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alp
     p.cnt_row = d_cnt_row.p; p.single_cnt = d_single_cnt.p;
     launch_em(p, em_tpb(), st);
     KB_CK(cudaGetLastError());
+    genes.run((uint32_t)nb, T, d_alpha.p, p.fstate, d_eff.p, in.per_sample_eff ? T : 0, nullptr, st);
     d_alpha.download(alpha_out.data() + (size_t)s0 * T, (size_t)nb * T, 0, st);
     d_emi.download(emi.data(), (size_t)2 * chunk, 0, st);
+    if (G) {
+      genes.counts.download(gene_counts_out->data() + (size_t)s0 * G, (size_t)nb * G, 0, st);
+      genes.tpm.download(gene_tpm_out->data() + (size_t)s0 * G, (size_t)nb * G, 0, st);
+    }
     KB_CK(cudaStreamSynchronize(st));
     for (int b = 0; b < nb; ++b) {
       rounds[s0 + b] = emi[b];
@@ -1700,7 +1752,7 @@ void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool wan
   // chunk touches fit ~2 GB of work space
   const uint64_t P = (uint64_t)S * B;
   auto rows_of = [&](uint64_t c) { return std::min<uint64_t>(S, (c + B - 2) / B + 1); };   // most rows c problems touch
-  const size_t per_prob = (size_t)nE * 4 + (size_t)T * 16 + (size_t)n_multi * 12 + 32;
+  const size_t per_prob = (size_t)nE * 4 + (size_t)T * 16 + (size_t)n_multi * 12 + 32 + TccGenes::per_problem(in);
   const size_t per_row = (size_t)nnz * 16 + (size_t)nE * 4 + (in.per_sample_eff ? (size_t)T * 8 : 0) + 16;
   auto fits = [&](uint64_t c) { return c * per_prob + rows_of(c) * per_row <= ((size_t)2 << 30); };
   uint64_t chunk = std::min<uint64_t>(P, KB_EM_MAX_BATCH);
@@ -1712,6 +1764,9 @@ void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool wan
   if (const char* s = getenv("KB_TCC_BS_CHUNK")) { const long v = atol(s); if (v > 0) chunk = std::min<uint64_t>(P, v); }   // tests
   chunk = std::min<uint64_t>(chunk, KB_EM_MAX_BATCH);
   const uint64_t rmax = rows_of(chunk);
+  const uint32_t G = in.n_genes;
+  TccGenes genes(T, in, chunk, st);
+  std::vector<double> gcounts(chunk * G), gtpm(chunk * G);
   DBuf<uint32_t> d_counts, d_samp, d_x0, d_cp_ec, d_wset, d_cnt_row;
   DBuf<unsigned long long> d_rowoff, d_cp_off, d_ndraws, d_chunkoff;
   DBuf<double> d_eff, d_mw, d_tw, d_alpha, d_norm, d_single_cnt, d_cp;
@@ -1771,15 +1826,21 @@ void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool wan
     p.cnt_row = d_cnt_row.p; p.single_cnt = d_single_cnt.p;
     launch_em(p, em_tpb(), st);
     KB_CK(cudaGetLastError());
+    genes.run((uint32_t)nb, T, d_alpha.p, p.fstate, d_eff.p, in.per_sample_eff ? T : 0, d_wset.p, st);
     d_alpha.download(est.data(), (size_t)nb * T, 0, st);
     d_emi.download(emi.data(), 2 * chunk, 0, st);
     if (want_samples) d_samp.download(samp.data(), (size_t)nb * nE, 0, st);
+    if (G) {
+      genes.counts.download(gcounts.data(), (size_t)nb * G, 0, st);
+      genes.tpm.download(gtpm.data(), (size_t)nb * G, 0, st);
+    }
     KB_CK(cudaStreamSynchronize(st));
     for (int b = 0; b < nb; ++b)
       if (emi[chunk + b] == 3)   // stop detected on the last allowed iteration: zero small alphas (EMAlgorithm.h:213-216)
         for (uint32_t t = 0; t < T; ++t)
           if (est[(size_t)b * T + t] < 1e-7 / 10.0) est[(size_t)b * T + t] = 0.0;
-    sink(g0, (uint32_t)nb, est.data(), emi.data(), want_samples ? samp.data() : nullptr);
+    sink(g0, (uint32_t)nb, est.data(), emi.data(), want_samples ? samp.data() : nullptr, G ? gcounts.data() : nullptr,
+         G ? gtpm.data() : nullptr);
   }
 }
 

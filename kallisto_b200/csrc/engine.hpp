@@ -328,13 +328,20 @@ struct TccInput {
   const uint32_t* counts = nullptr;
   const double* eff_lens = nullptr;     // n_targets, or n_samples x n_targets when per_sample_eff
   bool per_sample_eff = false;
+  // gene-level output (-g / -G): the gene of every target (-1: none), genes 0 .. n_genes - 1.  n_genes == 0: none is
+  // computed and nothing for it is allocated.
+  const int32_t* gene_of = nullptr;
+  uint32_t n_genes = 0;
 };
-std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out /* n_samples x n_targets */);
+// gene_counts_out / gene_tpm_out (n_samples x n_genes) are filled when in.n_genes > 0.
+std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out /* n_samples x n_targets */,
+                         std::vector<double>* gene_counts_out = nullptr, std::vector<double>* gene_tpm_out = nullptr);
 // The B bootstraps of every sample (src/main.cpp:3109-3178), problem g = sample * B + b, handed to `sink` chunk by chunk
-// in order: (first problem, count, est_counts count x n_targets, rounds, resampled counts count x n_ecs or nullptr).
-// Host memory is bounded by one chunk, whatever n_samples x B.
+// in order: (first problem, count, est_counts count x n_targets, rounds, resampled counts count x n_ecs or nullptr,
+// gene counts and gene TPM count x n_genes or nullptr without genes).  Host memory is bounded by one chunk, whatever
+// n_samples x B.
 using TccBootstrapSink = std::function<void(uint64_t first, uint32_t count, const double* est, const int* rounds,
-                                            const uint32_t* samples)>;
+                                            const uint32_t* samples, const double* gene_counts, const double* gene_tpm)>;
 void tcc_bootstrap(Index& ix, const TccInput& in, uint64_t seed, int B, bool want_samples, const TccBootstrapSink& sink);
 
 }  // namespace kb

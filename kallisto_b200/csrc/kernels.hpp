@@ -335,4 +335,22 @@ struct TccResampleArgs {
 };
 void launch_tcc_resample(const TccResampleArgs& a, cudaStream_t st);
 
+// quant-tcc gene-level output (src/main.cpp:3026-3058, plaintext_writer_gene src/PlaintextWriter.cpp:67-112): per problem,
+// tpm = counts_to_tpm(alpha, eff_lens), then for every transcript with alpha > 0 in increasing id, gene_counts[gene] +=
+// alpha and gene_tpm[gene] += tpm.  The genes come as a CSR of member transcripts in increasing id, so a (problem, gene)
+// thread adds in the reference's order; the total mass is a sequential sum in target order, one thread per problem.
+struct TccGeneArgs {
+  uint32_t nb, n_targets, n_genes;
+  const double* alpha;                  // nb x n_targets
+  const int* fstate;                    // nb: 3 -> alphas below 1e-8 count as 0 (the host zeroes them, EMAlgorithm.h:213-216)
+  const double* eff; uint64_t eff_stride;   // problem b's eff_lens: eff + (w_set ? w_set[b] : b) * eff_stride
+  const uint32_t* w_set;                // nb or nullptr
+  const uint32_t* g_off;                // n_genes + 1
+  const uint32_t* g_tid;                // member transcripts, increasing within a gene
+  double* total;                        // nb scratch: sum of alpha / eff_len
+  double* gene_counts;                  // nb x n_genes
+  double* gene_tpm;                     // nb x n_genes
+};
+void launch_tcc_genes(const TccGeneArgs& a, cudaStream_t st);
+
 }  // namespace kb

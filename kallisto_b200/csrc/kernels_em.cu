@@ -599,4 +599,54 @@ void launch_tcc_resample(const TccResampleArgs& a, cudaStream_t st) {
   tcc_resample_kernel<<<g, 256, 0, st>>>(a);
 }
 
+// Gene sums of quant-tcc.  Every operation is a separate IEEE double operation (no contraction), in the order of
+// counts_to_tpm (src/PlaintextWriter.cpp:5-27): tpm[i] = alpha[i] / eff[i]; total += tpm[i]; tpm[i] = (tpm[i] / total)
+// * 1e6.  The total is one sequential sum per problem, so it takes one thread per problem.
+namespace {
+__device__ __forceinline__ double gene_alpha(const TccGeneArgs& a, uint32_t b, uint32_t t) {
+  const double x = a.alpha[(size_t)b * a.n_targets + t];
+  return (a.fstate[b] == 3 && x < 1e-7 / 10.0) ? 0.0 : x;
+}
+__device__ __forceinline__ const double* gene_eff(const TccGeneArgs& a, uint32_t b) {
+  return a.eff + (size_t)(a.w_set ? a.w_set[b] : b) * a.eff_stride;
+}
+}  // namespace
+
+__global__ void tcc_gene_total_kernel(TccGeneArgs a) {
+  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.nb) return;
+  const double* eff = gene_eff(a, b);
+  double tot = 0.0;
+  for (uint32_t t = 0; t < a.n_targets; ++t) tot = __dadd_rn(tot, __ddiv_rn(gene_alpha(a, b, t), eff[t]));
+  a.total[b] = tot;
+}
+
+__global__ void __launch_bounds__(256) tcc_gene_sum_kernel(TccGeneArgs a) {
+  const uint64_t n = (uint64_t)a.nb * a.n_genes;
+  for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < n; w += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t b = (uint32_t)(w / a.n_genes), g = (uint32_t)(w % a.n_genes);
+    const double* eff = gene_eff(a, b);
+    const double tot = a.total[b];
+    double gc = 0.0, gt = 0.0;
+    for (uint32_t m = a.g_off[g]; m < a.g_off[g + 1]; ++m) {
+      const uint32_t t = a.g_tid[m];
+      const double x = gene_alpha(a, b, t);
+      if (x > 0.0) {
+        gc = __dadd_rn(gc, x);
+        gt = __dadd_rn(gt, __dmul_rn(__ddiv_rn(__ddiv_rn(x, eff[t]), tot), 1e6));
+      }
+    }
+    a.gene_counts[w] = gc;
+    a.gene_tpm[w] = gt;
+  }
+}
+
+void launch_tcc_genes(const TccGeneArgs& a, cudaStream_t st) {
+  if (a.nb == 0 || a.n_genes == 0) return;
+  tcc_gene_total_kernel<<<(a.nb + 127) / 128, 128, 0, st>>>(a);
+  const uint64_t n = (uint64_t)a.nb * a.n_genes;
+  const unsigned g = (unsigned)std::min<uint64_t>((uint64_t)device_sm_count() * 16, (n + 255) / 256);
+  tcc_gene_sum_kernel<<<g, 256, 0, st>>>(a);
+}
+
 }  // namespace kb

@@ -4,9 +4,14 @@
 EC counts.  Runs the CLI with --matrix-to-files --plaintext and reports the wall clock and the (sample, bootstrap) EMs
 per second, and the same bootstraps through the library with a callback that writes nothing (`library_seconds`: device
 work and transfers, no text); with --reference (and oracle/_ref/kallisto built) the unmodified `kallisto quant-tcc` on
-the same files.  Inputs and outputs live in a temporary directory.  Prints one JSON line.
+the same files.  With --genes, a transcript-to-gene map over the index's targets (genes of 1 to 7 consecutive
+transcripts, every 10th transcript in none) is written too, and the library (main EMs and bootstraps, alternately
+with and without the map, best of three each) and the CLI (alternately without and with `-g`, with and without
+`-b`, best of three each) are also timed with gene-level output; `gene_kernels_ms` is the device time of the gene
+kernels in one library call, from torch.profiler.  Inputs and
+outputs live in a temporary directory.  Prints one JSON line.
 
-    python tools/tcc_bootstrap_bench.py --samples 96 --bootstraps 100 --threads 16 [--reference]
+    python tools/tcc_bootstrap_bench.py --samples 96 --bootstraps 100 --threads 16 [--reference] [--genes]
 """
 import argparse
 import json
@@ -56,7 +61,32 @@ def run(exe, td, out, B, threads, extra=()):
     return dt
 
 
-def library_seconds(off, tids, rows, B, res):
+def write_t2g(td, names, seed):
+    """-> (gene of every target, n_genes); writes t2g.txt."""
+    rng = np.random.default_rng(seed)
+    gene_of = np.full(len(names), -1, np.int32)
+    lines, t, G = [], 0, 0
+    while t < len(names):
+        for i in range(t, min(len(names), t + int(rng.integers(1, 8)))):
+            if i % 10 != 9:
+                gene_of[i] = G
+                lines.append("%s\tG%05d\tname%d\n" % (names[i], G, G))
+            t = i + 1
+        G += 1
+    with open(os.path.join(td, "t2g.txt"), "w") as f:
+        f.writelines(lines)
+    return gene_of, G
+
+
+def gene_kernel_ms(fn):
+    """Device time of the gene pass (tcc_gene_*_kernel) in one call of fn, from torch.profiler's CUDA activity trace."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+    return round(sum(e.device_time_total for e in prof.key_averages() if "tcc_gene" in e.key) / 1000.0, 3)
+
+
+def library_seconds(off, tids, rows, B, res, td, genes):
     sys.path.insert(0, ROOT)
     import kallisto_b200 as K
     ix = K.KmerIndex(os.path.join(DATA, "transcripts.kidx"), device=0)
@@ -75,6 +105,29 @@ def library_seconds(off, tids, rows, B, res):
     res["library_seconds"] = round(time.perf_counter() - t0, 3)
     assert n[0] == len(rows) * (B + 1)
     T = ix.num_trans
+    if genes:
+        gmap = write_t2g(td, ix.target_names_, 2)
+        res["n_genes"] = gmap[1]
+        sets = [tuple(int(x) for x in tids[int(off[e]):int(off[e + 1])]) for e in range(len(off) - 1)]
+        sparse = [[(int(e), int(r[e])) for e in i] for r, i in zip(rows, ids)]
+        best = {}
+
+        def timed(key, fn):
+            t0 = time.perf_counter()
+            fn()
+            best[key] = min(best.get(key, 1e9), time.perf_counter() - t0)
+        K.tcc_run(ix, sets, sparse, eff, genes=gmap)                                 # warm-up
+        for _ in range(3):
+            timed("run", lambda: K.tcc_run(ix, sets, sparse, eff))
+            timed("run_genes", lambda: K.tcc_run(ix, sets, sparse, eff, genes=gmap))
+            timed("bs", lambda: K.tcc_bootstrap(ix, off, tids, ro, ec_ids, vals, eff, 42, B, on_chunk))
+            timed("bs_genes", lambda: K.tcc_bootstrap(ix, off, tids, ro, ec_ids, vals, eff, 42, B,
+                                                      lambda *a: None, genes=gmap))
+        res.update({"library_%s_seconds" % k: round(v, 4) for k, v in best.items()})
+        res["gene_kernels_ms"] = {
+            "run": gene_kernel_ms(lambda: K.tcc_run(ix, sets, sparse, eff, genes=gmap)),
+            "bootstrap": gene_kernel_ms(lambda: K.tcc_bootstrap(ix, off, tids, ro, ec_ids, vals, eff, 42, B,
+                                                                lambda *a: None, genes=gmap))}
     ix.close()
     return T
 
@@ -86,18 +139,27 @@ def main():
     ap.add_argument("--reads", type=int, default=2_000_000, help="fragments per sample")
     ap.add_argument("--threads", type=int, default=16)
     ap.add_argument("--reference", action="store_true", help="also time the reference (oracle/_ref/kallisto)")
+    ap.add_argument("--genes", action="store_true", help="also time gene-level output (-g)")
     a = ap.parse_args()
     R, B = a.samples, a.bootstraps
     res = dict(tool="tcc_bootstrap_bench", samples=R, bootstraps=B, reads_per_sample=a.reads, threads=a.threads)
     with tempfile.TemporaryDirectory() as td:
         off, tids, rows = write_inputs(td, R, a.reads, 1)
         res["n_ecs"] = len(off) - 1
-        res["n_targets"] = library_seconds(off, tids, rows, B, res)
+        res["n_targets"] = library_seconds(off, tids, rows, B, res, td, a.genes)
         run(CLI, td, "warm", 0, a.threads)                  # the same run without bootstraps: index load + main EMs
         t_main = run(CLI, td, "main", 0, a.threads)
         t = run(CLI, td, "kb", B, a.threads)
         res.update(seconds_without_bootstrap=round(t_main, 3), seconds=round(t, 3),
                    bootstrap_ems_per_s=round(R * B / max(1e-9, t - t_main), 1))
+        if a.genes:
+            # alternately without and with -g, best of three each
+            g = ["-g", os.path.join(td, "t2g.txt")]
+            best = {}
+            for i in range(3):
+                for key, b, extra in (("main", 0, []), ("main_g", 0, g), ("kb", B, []), ("kb_g", B, g)):
+                    best[key] = min(best.get(key, 1e9), run(CLI, td, "%s%d" % (key, i), b, a.threads, extra))
+            res.update(cli_best_of_3={k: round(v, 3) for k, v in best.items()})
         if a.reference and os.path.exists(REF):
             tr = run(REF, td, "ref", B, a.threads)
             res.update(reference_seconds=round(tr, 3), speedup=round(tr / t, 2))
