@@ -53,6 +53,26 @@ struct BatchWs {
   DBuf<uint8_t> d_skip;             // per fragment: holds a D-list k-mer (only when the index has a D-list)
 };
 
+// The per-problem device state of launch_em for up to `cap` problems (grow-only), and the one host-side driver of every
+// EM batch: launch() starts the problems from a uniform alpha with zeroed round counts, final states and change
+// counters; fetch() downloads their estimates and round counts and applies the state-3 zeroing.
+struct EmState {
+  DBuf<double> alpha, norm, single_cnt;
+  DBuf<uint32_t> cnt_row;
+  DBuf<int> emi;                    // rounds in [0, cap), final states in [cap, 2 cap)
+  DBuf<unsigned int> chcount, bar;  // two change counters per problem; the grid barrier's arrival counter
+  std::vector<int> h_emi;
+  size_t cap = 0;
+  void reserve(size_t nb, uint32_t T, size_t n_multi);
+  // p: the shared structure filled in by the caller (n_ec .. w_set, max_iter, min_rounds); its per-problem fields are
+  // pointed at this state.  `start` (optional) is recorded right before launch_em.  Returns what launch_em returns.
+  int launch(EmProblem& p, int nb, const uint32_t* counts, int threads_per_block, cudaStream_t st,
+             const EmCompWs* cw = nullptr, cudaEvent_t start = nullptr);
+  // Enqueues the download of p's nb x n_targets estimates and nb rounds behind whatever the caller enqueued since
+  // launch(), synchronises the stream once and zeroes the small estimates of problems that stopped in state 3.
+  void fetch(const EmProblem& p, double* alpha_out, int* rounds_out, cudaStream_t st);
+};
+
 struct EmWs {   // grow-only device workspace of run_em_device
   DBuf<uint32_t> used, scal, idx_in, order, handle, count, len, multi_len, is_multi, ec_off, m_off, multi_index;
   DBuf<unsigned long long> key_in, key_out;
@@ -60,18 +80,14 @@ struct EmWs {   // grow-only device workspace of run_em_device
   DBuf<uint32_t> ec_tid, multi_ec, m_rowoff, m_tid, m_row, m_iota, sortv, t_deg, t_off, t_midx;
   DBuf<uint32_t> minkey, ckey, cval, ckey_out, rlen;     // row order of the EM matrices (emprep_rows)
   DBuf<unsigned long long> k64_in, k64_out;              // CSC sort keys
-  DBuf<unsigned> bar;                                    // grid-barrier counter of em_kernel
-  DBuf<uint32_t> cnt_row;                                // row-ordered counts (launch_em fills them)
-  DBuf<double> single_cnt;
   // bootstrap over the same matrices (run_bootstrap_device)
   DBuf<uint32_t> bs_counts, bs_x0;
-  DBuf<double> bs_alpha, bs_norm, bs_cp;
-  DBuf<int> bs_emi;
-  DBuf<unsigned int> bs_ch;
-  DBuf<double> m_w, t_w, eff, alpha, norm;
+  DBuf<double> bs_cp;
+  DBuf<double> m_w, t_w, eff;
   DBuf<int32_t> t_single;
-  DBuf<int> emi;
-  DBuf<unsigned int> chcount;
+  EmState em;                                            // per-problem state of run_em_device and the bootstrap
+  // the shared structure of the EM matrices run_em_device built here (n_ec ECs, n_multi of them with >= 2 targets)
+  EmProblem problem(uint32_t n_ec, uint32_t T, uint32_t n_multi, int max_iter, int min_rounds) const;
   // component layout of the single-problem EM (EmCompWs, kernels.hpp)
   DBuf<uint32_t> c_parent, c_rfirst, c_iota, c_tkey, c_tid, c_tloc, c_rcomp, c_rkey, c_rid, c_rloc, c_rcnt, c_rlen, c_roff;
   DBuf<uint32_t> c_tlen, c_toff, c_st0, c_sr0;

@@ -514,6 +514,17 @@ __device__ __forceinline__ uint32_t powmod(uint32_t a, uint64_t e) {
   }
   return r;
 }
+// The next draw of generate_canonical<double, 53> from engine state x: two engine steps, then
+// (x1 - 1 + (x2 - 1) R) / R^2 with R = 2^31 - 2, kept below 1.0.
+__device__ __forceinline__ double next_draw(uint32_t& x) {
+  const double R = 2147483646.0;
+  x = mulmod(x, 16807u);
+  const double u0 = (double)(x - 1);
+  x = mulmod(x, 16807u);
+  const double u1 = (double)(x - 1);
+  const double u = __ddiv_rn(__dadd_rn(u0, __dmul_rn(u1, R)), __dmul_rn(R, R));
+  return u >= 1.0 ? 0.99999999999999988897769753748 : u;   // nextafter(1.0, 0.0)
+}
 constexpr int kDrawsPerThread = 64;
 }
 
@@ -525,15 +536,8 @@ __global__ void __launch_bounds__(256) resample_kernel(ResampleArgs a) {
   const uint64_t d1 = min(a.n_draws, d0 + kDrawsPerThread);
   uint32_t x = mulmod(a.x0[b], powmod(16807u, 2 * d0));
   uint32_t* samp = a.samp + (size_t)b * a.n_ec;
-  const double R = 2147483646.0;
-  const double RR = __dmul_rn(R, R);
   for (uint64_t d = d0; d < d1; ++d) {
-    x = mulmod(x, 16807u);
-    const double u0 = (double)(x - 1);
-    x = mulmod(x, 16807u);
-    const double u1 = (double)(x - 1);
-    double u = __ddiv_rn(__dadd_rn(u0, __dmul_rn(u1, R)), RR);
-    if (u >= 1.0) u = 0.99999999999999988897769753748;   // nextafter(1.0, 0.0)
+    const double u = next_draw(x);
     // std::lower_bound(cp.begin(), cp.end(), u): first index with cp[idx] >= u
     uint32_t lo = 0, hi = a.n_ec;
     while (lo < hi) {
@@ -556,8 +560,6 @@ void launch_resample(const ResampleArgs& a, cudaStream_t st) {
 // hold from 0 to tens of millions of draws, so the problems are not a grid dimension: every thread takes 64-draw
 // chunks of one flat list (grid-stride) and finds its problem by binary search in the chunk prefix sum.
 __global__ void __launch_bounds__(256) tcc_resample_kernel(TccResampleArgs a) {
-  const double R = 2147483646.0;
-  const double RR = __dmul_rn(R, R);
   for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < a.n_chunks; w += (uint64_t)gridDim.x * blockDim.x) {
     uint32_t lo = 0, hi = a.nb;                 // last problem with chunk_off[p] <= w
     while (hi - lo > 1) {
@@ -574,12 +576,7 @@ __global__ void __launch_bounds__(256) tcc_resample_kernel(TccResampleArgs a) {
     uint32_t* samp = a.samp + (size_t)p * a.n_ec;
     uint32_t x = mulmod(a.x0[b], powmod(16807u, 2 * d0));
     for (uint64_t d = d0; d < d1; ++d) {
-      x = mulmod(x, 16807u);
-      const double u0 = (double)(x - 1);
-      x = mulmod(x, 16807u);
-      const double u1 = (double)(x - 1);
-      double u = __ddiv_rn(__dadd_rn(u0, __dmul_rn(u1, R)), RR);
-      if (u >= 1.0) u = 0.99999999999999988897769753748;   // nextafter(1.0, 0.0)
+      const double u = next_draw(x);
       // lower_bound over the row's table: its last entry is 1.0 > u, so the search ends inside the table
       uint64_t l = t0, h = t1;
       while (l < h) {
