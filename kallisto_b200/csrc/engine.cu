@@ -559,7 +559,7 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ra.group = resolve_group_;
 
   int tpb = opt_.threads_per_block;
-  const size_t per_thread = (size_t)4 * (KB_MAX_E + 3 + 4 * ba.nb);   // match_kernel's shared memory per lane
+  const size_t per_thread = 4 * match_lane_words(ba.nb);   // match_kernel's shared memory per lane
   while (tpb > 32 && per_thread * tpb > 200 * 1024) tpb >>= 1;
   if (per_thread * tpb > 200 * 1024) throw Error("kallisto_b200: read too long for the short-read kernel");
   cudaEvent_t* ev = nullptr;

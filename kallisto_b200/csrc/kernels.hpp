@@ -74,6 +74,10 @@ static constexpr int KB_Q_STRIDE = 2 + KB_MAX_E + 6;   // frag, n|flags, handles
 static constexpr int KB_SPILL = 112;                   // a fragment may hit KB_MAX_E + KB_SPILL = 128 distinct EC sets
 static constexpr int KB_QBIG_STRIDE = 2 + KB_MAX_E + KB_SPILL + 6;
 static constexpr uint32_t KB_QBIG_CAP = 1u << 16;      // wide-queue entries per batch
+// match_kernel's shared memory per lane, in 32-bit words: the handle tuple, 6 words per lookup chain (first hit, the
+// reference's nextPos, the second hit of a jump), then the 2-bit bases of both mates (2 x 2 nb words)
+static constexpr int KB_CHAIN_WORDS = 6;
+__host__ __device__ constexpr size_t match_lane_words(uint32_t nb) { return (size_t)KB_MAX_E + 2 * KB_CHAIN_WORDS + 4 * (size_t)nb; }
 
 struct ResolveArgs {
   uint32_t* scratch;        // per lane group: scratch_stride entries
