@@ -34,6 +34,8 @@ struct DBuf {
   DBuf& operator=(const DBuf&) = delete;
   ~DBuf() { release(); }
   void alloc(size_t count);
+  // grow-only: at least `need` elements (contents are lost when it grows); `slack` over-allocates by that fraction
+  void grow(size_t need, double slack = 0.0) { if (n < need) alloc(need + (size_t)((double)need * slack)); }
   void release();
   void upload(const T* src, size_t count, cudaStream_t st = 0);
   void download(T* dst, size_t count, size_t offset = 0, cudaStream_t st = 0) const;
@@ -73,7 +75,7 @@ struct EmState {
   void fetch(const EmProblem& p, double* alpha_out, int* rounds_out, cudaStream_t st);
 };
 
-struct EmWs {   // grow-only device workspace of run_em_device
+struct EmWs {   // grow-only device workspace of Quant::number_ecs and of what run_em_device builds on its numbering
   DBuf<uint32_t> used, scal, idx_in, order, handle, count, len, multi_len, is_multi, ec_off, m_off, multi_index;
   DBuf<unsigned long long> key_in, key_out;
   DBuf<uint8_t> tmp;
@@ -86,6 +88,11 @@ struct EmWs {   // grow-only device workspace of run_em_device
   DBuf<double> m_w, t_w, eff;
   DBuf<int32_t> t_single;
   EmState em;                                            // per-problem state of run_em_device and the bootstrap
+  // The two sizings (slack: see DBuf::grow): what number_ecs touches for n ECs, and the EM matrices and single-problem
+  // state of n ECs (n_multi of them with >= 2 targets, nnz entries in those) over T targets.  ec_tid, the EC table's
+  // entries, is sized by whoever fills it.
+  void reserve_numbering(size_t dict_cap, size_t n, double slack);
+  void reserve_matrices(size_t n, uint32_t T, size_t n_multi, size_t nnz, double slack);
   // the shared structure of the EM matrices run_em_device built here (n_ec ECs, n_multi of them with >= 2 targets)
   EmProblem problem(uint32_t n_ec, uint32_t T, uint32_t n_multi, int max_iter, int min_rounds) const;
   // component layout of the single-problem EM (EmCompWs, kernels.hpp)
@@ -98,6 +105,14 @@ struct EmWs {   // grow-only device workspace of run_em_device
   DBuf<uint8_t> c_tmp;
   // grows the buffers to T transcripts, R rows, nnz entries and max_iter rounds and hands them out
   EmCompWs comp(uint32_t T, uint32_t R, size_t nnz, int max_iter);
+};
+
+// What Quant::number_ecs found: n ECs with n_entries transcript ids in all, n_multi of them with >= 2 transcripts and
+// multi_entries ids in those; `prep` points at their handle / count / len / offsets in the EmWs (ec_tid and the
+// matrices are for the caller to size and fill).
+struct EcNumbering {
+  uint32_t n = 0, n_entries = 0, multi_entries = 0, n_multi = 0;
+  EmPrep prep{};
 };
 
 class Index {
@@ -215,7 +230,8 @@ class Quant {
   const int32_t* device_handles() const { return bws_->d_handles.p; }
   void sync();
 
-  // MasterProcessor tail flush + EC id assignment.
+  // MasterProcessor tail flush + EC id assignment: the table export_prepare lays out on the device (ids from
+  // number_ecs), downloaded.
   const EcTable& finalize_ecs();
   const std::vector<uint32_t>& flens() const { return flens_; }
   void set_flens(const uint32_t* f);     // e.g. after an all-reduce across ranks
@@ -227,7 +243,7 @@ class Quant {
   // Same result, EC table built and kept on the device (the `quant` fast path).
   EmResult run_em_device(const std::vector<double>& fl_trunc, int max_iter = 10000, int min_rounds = 50);
   // ---- multi-GPU: ship this rank's equivalence classes to another rank / fold another rank's in ----
-  // export_prepare numbers the ECs (first occurrence) and lays the table out on the device; returns
+  // export_prepare numbers the ECs (number_ecs) and lays the table out on the device; returns
   // {n_sets, n_entries}.  export_copy then fills caller-provided DEVICE buffers (e.g. torch tensors
   // about to go through NCCL): off[n_sets+1], tids[n_entries], counts[n_sets], first[n_sets].
   void export_prepare(uint32_t* n_sets, uint32_t* n_entries);
@@ -276,6 +292,9 @@ class Quant {
   void run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
                  uint32_t max_read_len, const uint8_t* d_bases2 = nullptr, const uint32_t* d_off2 = nullptr);
   void check_device_errors();
+  // The one EC numbering of every path: the used sets, ids in order of first occurrence, with their handles, counts,
+  // lengths and table offsets in emws_.  Synchronises the stream.
+  EcNumbering number_ecs();
   void apply_l2_window();
   uint32_t bus_core(const uint8_t* const* db, const uint32_t* const* dofs, uint32_t n_sets, uint32_t maxlen);
 
