@@ -26,7 +26,36 @@
 #define KB_MATCH_MIN_BLOCKS 3
 #endif
 
+#ifdef KB_MATCH_STATS
+#include <cstdio>
+#endif
+
 namespace kb {
+
+#ifdef KB_MATCH_STATS
+// Instrumented build (-DKB_MATCH_STATS, tools/match_stats.py): per-launch counters of match_kernel, printed to stderr
+// by launch_pseudoalign.  The counters and the host synchronisation slow the kernel; only their ratios mean something.
+enum : int {
+  MS_WARP_ITERS, MS_SERVICE_ROUNDS, MS_LANE_ITERS, MS_CHAIN_ITERS,
+  MS_MAIN_HIT, MS_MAIN_MISS_FILTER, MS_MAIN_MISS_SLOT, MS_JUMP, MS_MIDDLE, MS_BACKOFF, MS_COLLISION,
+  MS_CYCLES_LOOKUP, MS_CYCLES_SERVICE,
+  MS_RUN_HIST, MS_N = MS_RUN_HIST + 9     // MAIN miss runs of 1, 2, 3, 4, 5-8, 9-16, 17-32, 33-64, 65+ positions
+};
+__device__ unsigned long long kb_match_stats[MS_N];
+static const char* const kMatchStatNames[MS_N] = {
+  "warp_iters", "service_rounds", "lane_iters", "chain_iters",
+  "main_hit", "main_miss_filter", "main_miss_slot", "jump", "middle", "backoff", "collision",
+  "cycles_lookup", "cycles_service",
+  "run_1", "run_2", "run_3", "run_4", "run_5_8", "run_9_16", "run_17_32", "run_33_64", "run_65_"};
+__device__ __forceinline__ int run_bin(int n) {
+  return n <= 4 ? n - 1 : (n <= 8 ? 4 : (n <= 16 ? 5 : (n <= 32 ? 6 : (n <= 64 ? 7 : 8))));
+}
+#define KB_MS(i, n) (ms[i] += (unsigned long long)(n))
+#define KB_MS_ONLY(x) x
+#else
+#define KB_MS(i, n) ((void)0)
+#define KB_MS_ONLY(x)
+#endif
 
 namespace {
 
@@ -348,6 +377,12 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
   uint64_t canon[2] = {0, 0}, slot[2] = {0, 0};
   uint32_t n_probes = 0, n_visits = 0, n_memo = 0;   // per-lane totals: touched once per fragment (they live in local memory)
   uint32_t pv = 0;          // hot-loop counter of the current fragment: lookups in the low half, slot visits in the high half
+#ifdef KB_MATCH_STATS
+  unsigned long long ms[MS_N] = {};
+  int run[2] = {0, 0};      // current MAIN miss run of each chain, in positions
+  long long t_mark = clock64();
+  auto end_run = [&](int c) { if (run[c] > 0) { KB_MS(MS_RUN_HIST + run_bin(run[c]), 1); run[c] = 0; } };
+#endif
   // view of mate c of the lane's fragment
   auto view = [&](int c) {
     ReadView rv;
@@ -361,14 +396,25 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     return rv;
   };
 
+  KB_MS_ONLY(bool in_service = true;)
   for (;;) {
+#ifdef KB_MATCH_STATS
+    {
+      const long long t_now = clock64();
+      KB_MS(in_service ? MS_CYCLES_SERVICE : MS_CYCLES_LOOKUP, t_now - t_mark);
+      t_mark = t_now;
+    }
+#endif
     // ------------------------------------------------------------------ service round
     const bool done = st[0] == S_FIN && st[1] == S_FIN;
     const unsigned fin = __ballot_sync(0xFFFFFFFFu, done);
     const unsigned idle = fin | __ballot_sync(0xFFFFFFFFu, st[0] == S_EMPTY);
     const bool work_left = next < end;
     if (idle == 0xFFFFFFFFu && fin == 0 && !work_left) break;
+    KB_MS_ONLY(in_service = false;)
     if (idle == 0xFFFFFFFFu || (work_left && __popc(idle) >= ba.refill_min)) {
+      KB_MS(MS_SERVICE_ROUNDS, 1);
+      KB_MS_ONLY(in_service = true;)
       if (done) {
         n_probes += pv & 0xFFFFu;     // a fragment executes at most a few hundred lookups
         n_visits += pv >> 16;
@@ -565,7 +611,9 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     }
     // ------------------------------------------------------------------ one lookup per live chain
     const bool live[2] = {st[0] <= S_BACKOFF, st[1] <= S_BACKOFF};
+    KB_MS(MS_WARP_ITERS, 1);
     if (live[0] || live[1]) {
+      KB_MS(MS_LANE_ITERS, 1);
       // keys of both chains and their presence-filter words (L2 resident) before either is used
       uint32_t fword[2] = {0xFFFFFFFFu, 0xFFFFFFFFu}, fbit[2] = {0, 0};
 #pragma unroll
@@ -580,8 +628,10 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
           slot[c] = hsh & ix.mask;
           need_prep[c] = false;
           ++pv;
-          // a clear bit means the k-mer is not in the index -- no HBM sector is touched
-          if (ix.filter) {
+          // a clear bit means the k-mer is not in the index -- no HBM sector is touched.  The jump target and the
+          // middle k-mer lie in the EC block of the hit before them and are nearly always present: their slot is
+          // loaded without the filter word, which would only add an L2 round trip and an L2 request
+          if (ix.filter && (st[c] == S_MAIN || st[c] == S_BACKOFF)) {
             const uint32_t fidx = (uint32_t)(hsh >> 32) & ix.filter_mask;
             fword[c] = __ldg(ix.filter + (fidx >> 5));
             fbit[c] = fidx & 31;
@@ -602,12 +652,22 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         if (!live[c]) continue;
+        KB_MS(MS_CHAIN_ITERS, 1);
         const uint64_t key = (uint64_t)v[c][0] | ((uint64_t)v[c][1] << 32);
         if (key != canon[c] && key != KB_EMPTY_KEY) {
           slot[c] = (slot[c] + 1) & ix.mask;        // linear probing: one more iteration
+          KB_MS(MS_COLLISION, 1);
           continue;
         }
         const bool f = key == canon[c];
+#ifdef KB_MATCH_STATS
+        if (st[c] == S_MAIN) {
+          if (f) { KB_MS(MS_MAIN_HIT, 1); end_run(c); }
+          else { KB_MS(((fword[c] >> fbit[c]) & 1u) ? MS_MAIN_MISS_SLOT : MS_MAIN_MISS_FILTER, 1); ++run[c]; }
+        } else {
+          KB_MS(st[c] == S_JUMP ? MS_JUMP : (st[c] == S_MIDDLE ? MS_MIDDLE : MS_BACKOFF), 1);
+        }
+#endif
         // hit fields: v[2] unitig, v[3] blk, v[4] ec (set handle), v[5] dist|flag, v[6] lb, v[7] ub
         const uint32_t r_unitig = v[c][2], r_ec = v[c][4];
         const bool r_strand = (is_canon[c] == ((v[c][5] >> 31) != 0));
@@ -696,6 +756,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
           else { st[c] = to_backoff ? S_BACKOFF : S_MAIN; need_prep[c] = true; }
         }
         if (end_chain) st[c] = S_FIN;
+        KB_MS_ONLY(if (st[c] == S_FIN) end_run(c);)
       }
     }
   }
@@ -712,6 +773,15 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     atomicAdd(&dd.stats[3], (unsigned long long)n_visits);
     if (n_memo) atomicAdd(&dd.stats[2], (unsigned long long)n_memo);
   }
+#ifdef KB_MATCH_STATS
+  for (int i = 0; i < MS_N; ++i) {
+    const bool per_warp = i == MS_WARP_ITERS || i == MS_SERVICE_ROUNDS || i == MS_CYCLES_LOOKUP || i == MS_CYCLES_SERVICE;
+    unsigned long long x = ms[i];
+    if (!per_warp)
+      for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xFFFFFFFFu, x, o);
+    if (lane == 0 && x) atomicAdd(&kb_match_stats[i], x);
+  }
+#endif
 }
 
 namespace {
@@ -1045,7 +1115,22 @@ void launch_pseudoalign(const DevIndex& ix, const DevDict& dd, const BatchArgs& 
     if (ix.dfk && ba.skip_w) dlist_scan_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ix, ba, n_reads);
   }
   if (ev) cudaEventRecord(ev[1], st);
+#ifdef KB_MATCH_STATS
+  void* ms_dev = nullptr;
+  cudaGetSymbolAddress(&ms_dev, kb_match_stats);
+  cudaMemsetAsync(ms_dev, 0, sizeof(unsigned long long) * MS_N, st);
+#endif
   match_kernel<<<blocks, tpb, smem, st>>>(ix, dd, ba);
+#ifdef KB_MATCH_STATS
+  {
+    unsigned long long h[MS_N];
+    cudaMemcpyAsync(h, ms_dev, sizeof(h), cudaMemcpyDeviceToHost, st);
+    cudaStreamSynchronize(st);
+    fprintf(stderr, "kb_match_stats {\"n_frag\": %u", ba.n_frag);
+    for (int i = 0; i < MS_N; ++i) fprintf(stderr, ", \"%s\": %llu", kMatchStatNames[i], h[i]);
+    fprintf(stderr, "}\n");
+  }
+#endif
   if (ev) cudaEventRecord(ev[2], st);
   switch (ra.group) {      // lanes per fragment (engine.cu: KB_RESOLVE_G, default 32)
     case 4: resolve_kernel<4><<<(ra.n_warps * 4 + 127) / 128, 128, 0, st>>>(ix, dd, ba, ra); break;
