@@ -109,6 +109,7 @@ typedef struct kb_kernel_timings {
   double bs_resample_ms, bs_em_ms;   /* last kb_bootstrap_run: multinomial resampling, batched EM (CUDA events) */
   double pack_ms;             /* pack_kernel (+ dlist_scan_kernel with a D-list index), same launches as match_ms */
   uint64_t em_comp_blocks;    /* last single-problem EM: blocks of the per-component kernel, 0 for the grid-wide kernel */
+  uint64_t em_comp_resident;  /* ... 1 when that kernel held the entries in shared memory, 0 when it streamed them */
 } kb_kernel_timings;
 int kb_quant_enable_timing(kb_quant* q, int on);
 int kb_quant_get_timings(kb_quant* q, kb_kernel_timings* out);

@@ -43,7 +43,7 @@ class kb_kernel_timings(C.Structure):
     _fields_ = [("match_ms", C.c_double), ("resolve_ms", C.c_double), ("em_ms", C.c_double), ("em_prep_ms", C.c_double),
                 ("match_launches", C.c_uint64), ("resolve_launches", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("bs_resample_ms", C.c_double), ("bs_em_ms", C.c_double), ("pack_ms", C.c_double),
-                ("em_comp_blocks", C.c_uint64)]
+                ("em_comp_blocks", C.c_uint64), ("em_comp_resident", C.c_uint64)]
 
 
 class kb_bus_substr(C.Structure):

@@ -194,6 +194,7 @@ int kb_quant_get_timings(kb_quant* q, kb_kernel_timings* out) {
     out->bs_em_ms = q->q->last_bs_em_ms;
     out->pack_ms = t.pack_ms;
     out->em_comp_blocks = (uint64_t)q->q->last_em_comp_blocks;
+    out->em_comp_resident = q->q->last_em_comp_resident ? 1 : 0;
   });
 }
 

@@ -379,7 +379,7 @@ void Quant::reserve_em(size_t n_ecs, size_t nnz) {
   w.reserve_numbering(ix_.dict_cap, n_ecs, 0.0);
   w.ec_tid.grow(std::max<size_t>(1, nnz));
   w.reserve_matrices(n_ecs, T, n_ecs, nnz, 0.0);
-  w.comp(T, (uint32_t)std::min<size_t>(n_ecs, UINT32_MAX - 1), nnz, 10000);
+  w.comp(T, (uint32_t)std::min<size_t>(n_ecs, UINT32_MAX - 1), nnz, 10000, nullptr);
 }
 
 void EmWs::reserve_numbering(size_t dict_cap, size_t n, double slack) {
@@ -403,14 +403,14 @@ void EmWs::reserve_matrices(size_t n, uint32_t T, size_t n_multi, size_t nnz, do
   em.reserve(1, T, n_multi);
 }
 
-EmCompWs EmWs::comp(uint32_t T, uint32_t R, size_t nnz, int max_iter) {
+EmCompWs EmWs::comp(uint32_t T, uint32_t R, size_t nnz, int max_iter, const double* eff) {
   const size_t t1 = (size_t)T + 1, r1 = (size_t)R + 1, nz = std::max<size_t>(1, nnz);
   const size_t slices = (size_t)device_sm_count() + 1;
   c_parent.grow(t1); c_rfirst.grow(t1); c_iota.grow(std::max(t1, r1)); c_tkey.grow(t1); c_tid.grow(t1); c_tloc.grow(t1);
   c_rcomp.grow(r1); c_rkey.grow(r1); c_rid.grow(r1); c_rloc.grow(r1); c_rcnt.grow(r1); c_rlen.grow(r1); c_roff.grow(r1);
   c_tlen.grow(t1); c_toff.grow(t1); c_st0.grow(slices); c_sr0.grow(slices);
   c_csize.grow(t1); c_cstart.grow(t1); c_tsize.grow(t1); c_tscan.grow(t1); c_stats.grow(8);
-  c_rtid.grow(nz); c_trow.grow(nz); c_rw.grow(nz); c_tw.grow(nz); c_tsingle.grow(t1);
+  c_rtid.grow(nz); c_trow.grow(nz); c_rw.grow(nz); c_tw.grow(nz); c_tsingle.grow(t1); c_teff.grow(t1);
   c_sync.grow(2 * (size_t)std::max(1, max_iter));
   c_tmp.grow(emcomp_tmp_bytes(T, R));
   EmCompWs c{};
@@ -419,6 +419,7 @@ EmCompWs EmWs::comp(uint32_t T, uint32_t R, size_t nnz, int max_iter) {
   c.rcomp = c_rcomp.p; c.rkey = c_rkey.p; c.r_id = c_rid.p; c.rloc = c_rloc.p; c.r_cnt = c_rcnt.p; c.r_len = c_rlen.p;
   c.r_off = c_roff.p; c.r_tid = c_rtid.p; c.r_w = c_rw.p; c.t_single = c_tsingle.p; c.t_len = c_tlen.p; c.t_off = c_toff.p;
   c.t_row = c_trow.p; c.t_w = c_tw.p; c.s_t0 = c_st0.p; c.s_r0 = c_sr0.p; c.stats = c_stats.p; c.sync = c_sync.p;
+  c.eff = eff; c.t_eff = c_teff.p;
   c.sync_rounds = (int)(c_sync.n / 2);
   c.max_slices = (int)(std::min(c_st0.n, c_sr0.n) - 1);
   c.tmp = c_tmp.p;
@@ -1050,7 +1051,7 @@ void EmState::reserve(size_t nb, uint32_t T, size_t n_multi) {
 }
 
 int EmState::launch(EmProblem& p, int nb, const uint32_t* counts, int threads_per_block, cudaStream_t st,
-                    const EmCompWs* cw, cudaEvent_t start) {
+                    const EmCompWs* cw, cudaEvent_t start, bool* comp_resident) {
   const uint32_t T = p.n_targets;
   reserve((size_t)nb, T, p.n_multi);
   launch_fill_f64(alpha.p, (uint64_t)nb * T, 1.0 / T, st);   // uniform start (EMAlgorithm.h:38)
@@ -1059,7 +1060,7 @@ int EmState::launch(EmProblem& p, int nb, const uint32_t* counts, int threads_pe
   p.nb = nb; p.counts = counts; p.alpha = alpha.p; p.norm = norm.p; p.cnt_row = cnt_row.p; p.single_cnt = single_cnt.p;
   p.rounds = emi.p; p.fstate = emi.p + cap; p.chcount = chcount.p; p.bar = bar.p;
   if (start) KB_CK(cudaEventRecord(start, st));
-  const int blocks = launch_em(p, threads_per_block, st, cw);
+  const int blocks = launch_em(p, threads_per_block, st, cw, comp_resident);
   KB_CK(cudaGetLastError());
   return blocks;
 }
@@ -1112,9 +1113,9 @@ EmResult Quant::run_em(const EcTable& ecs, const std::vector<double>& fl_trunc, 
   EmProblem p = sh.problem(max_iter, min_rounds);
   p.m_w = d_mw.p; p.t_w = d_tw.p;
   EventGuard e0, e1;
-  const EmCompWs cw = emws_->comp(T, p.n_multi, sh.nnz, max_iter);
+  const EmCompWs cw = emws_->comp(T, p.n_multi, sh.nnz, max_iter, d_eff.p);
   EmState s;
-  last_em_comp_blocks = s.launch(p, 1, d_counts.p, 256, st, &cw, e0.e);
+  last_em_comp_blocks = s.launch(p, 1, d_counts.p, 256, st, &cw, e0.e, &last_em_comp_resident);
   KB_CK(cudaEventRecord(e1.e, st));
   r.alpha.resize(T);
   s.fetch(p, r.alpha.data(), &r.rounds, st);
@@ -1202,12 +1203,12 @@ EmResult Quant::run_em_device(const std::vector<double>& fl_trunc, int max_iter,
   KB_CK(cudaGetLastError());
   // ---- EM
   EmProblem p = w.problem(n, T, n_multi, max_iter, min_rounds);
-  const EmCompWs cw = w.comp(T, n_multi, nnz, max_iter);
+  const EmCompWs cw = w.comp(T, n_multi, nnz, max_iter, w.eff.p);
   mark("fill launches + uploads");
   // collect_used, gather_used, ec_meta, multi_compact, row_len, ec_fill, csc_fill, stats, fill_i32, fill_f64,
   // em_gather_counts + em_kernel
   n_kernel_launches += 11 + 1;
-  last_em_comp_blocks = w.em.launch(p, 1, w.count.p, em_tpb(), st, &cw, e1.e);
+  last_em_comp_blocks = w.em.launch(p, 1, w.count.p, em_tpb(), st, &cw, e1.e, &last_em_comp_resident);
   KB_CK(cudaEventRecord(e2.e, st));
   unsigned long long s2[2] = {0, 0};
   w.key_in.download(s2, 2, 0, st);

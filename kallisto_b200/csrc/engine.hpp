@@ -69,7 +69,7 @@ struct EmState {
   // p: the shared structure filled in by the caller (n_ec .. w_set, max_iter, min_rounds); its per-problem fields are
   // pointed at this state.  `start` (optional) is recorded right before launch_em.  Returns what launch_em returns.
   int launch(EmProblem& p, int nb, const uint32_t* counts, int threads_per_block, cudaStream_t st,
-             const EmCompWs* cw = nullptr, cudaEvent_t start = nullptr);
+             const EmCompWs* cw = nullptr, cudaEvent_t start = nullptr, bool* comp_resident = nullptr);
   // Enqueues the download of p's nb x n_targets estimates and nb rounds behind whatever the caller enqueued since
   // launch(), synchronises the stream once and zeroes the small estimates of problems that stopped in state 3.
   void fetch(const EmProblem& p, double* alpha_out, int* rounds_out, cudaStream_t st);
@@ -100,11 +100,12 @@ struct EmWs {   // grow-only device workspace of Quant::number_ecs and of what r
   DBuf<uint32_t> c_tlen, c_toff, c_st0, c_sr0;
   DBuf<unsigned long long> c_csize, c_cstart, c_tsize, c_tscan, c_stats;
   DBuf<uint16_t> c_rtid, c_trow;
-  DBuf<double> c_rw, c_tw, c_tsingle;
+  DBuf<double> c_rw, c_tw, c_tsingle, c_teff;
   DBuf<unsigned> c_sync;
   DBuf<uint8_t> c_tmp;
-  // grows the buffers to T transcripts, R rows, nnz entries and max_iter rounds and hands them out
-  EmCompWs comp(uint32_t T, uint32_t R, size_t nnz, int max_iter);
+  // grows the buffers to T transcripts, R rows, nnz entries and max_iter rounds and hands them out; `eff`: the
+  // effective lengths the weights were formed from (EmCompWs::eff)
+  EmCompWs comp(uint32_t T, uint32_t R, size_t nnz, int max_iter, const double* eff);
 };
 
 // What Quant::number_ecs found: n ECs with n_entries transcript ids in all, n_multi of them with >= 2 transcripts and
@@ -283,6 +284,7 @@ class Quant {
   double last_em_seconds = 0, last_prep_seconds = 0, last_bs_resample_ms = 0, last_bs_em_ms = 0;
   uint64_t n_kernel_launches = 0;   // launches of this library's own kernels by this run (CUB's are not counted)
   int last_em_comp_blocks = 0;      // last single-problem EM: blocks of em_component_kernel, 0 for the grid-wide kernels
+  bool last_em_comp_resident = false;   // ... and whether that kernel held the entries in shared memory
   // filled by run_em_device
   bool dev_stats_valid_ = false, dev_problem_valid_ = false;
   uint32_t dev_n_multi_ = 0;

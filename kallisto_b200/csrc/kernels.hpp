@@ -203,8 +203,13 @@ struct EmCompWs {
   double* t_w;                    // nnz
   uint32_t* s_t0;                 // slices + 1: first pos of each slice
   uint32_t* s_r0;                 // slices + 1: first row pos of each slice
+  const double* eff;              // T, by transcript id: effective lengths the weights were formed from; nullptr: the
+                                  //    resident kernel is off
+  double* t_eff;                  // T: effective length of the transcript at each pos
   unsigned long long* stats;      // 8: [0] total size, [1] slice target size, [2] slices, [3] largest component,
-                                  //    [4] largest slice's shared memory (bytes)
+                                  //    [4] largest slice's shared memory (bytes), [5] entries whose weight
+                                  //    emcomp_weight does not rebuild bit for bit, [6] largest slice's shared memory
+                                  //    in the resident layout (bytes)
   unsigned* sync;                 // 2 x sync_rounds: per round, blocks that changed an estimate, blocks that arrived
   int sync_rounds;
   int max_slices;                 // capacity of s_t0 / s_r0 minus one
@@ -216,17 +221,36 @@ struct EmCompWs {
 __host__ __device__ inline unsigned long long emcomp_smem_bytes(uint32_t nt, uint32_t nr) {
   return 20ull * nt + 16ull * nr + 8;
 }
+// The resident layout of the same slice with ne entries: also the effective length and its reciprocal per transcript
+// (doubles), and every entry's two 16-bit indices; the weights are rebuilt from the counts (emcomp_weight).
+__host__ __device__ inline unsigned long long emcomp_resident_bytes(uint32_t nt, uint32_t nr, unsigned long long ne) {
+  return emcomp_smem_bytes(nt, nr) + 16ull * nt + 4ull * ne;
+}
+// The weight of an entry, count c / eff, from y = __drcp_rn(eff): q = c y is within an ulp of c / eff, the residual
+// c - q eff is exact in one fma, and q + r y is then the correctly rounded quotient (Markstein), i.e.
+// __ddiv_rn(c, eff), which is how the weights are formed (calc_weights).  emcomp_cut checks every entry anyway.
+__device__ __forceinline__ double emcomp_weight(double c, double eff, double y) {
+  const double q = __dmul_rn(c, y);
+  return __fma_rn(__fma_rn(-q, eff, c), y, q);
+}
 size_t emcomp_tmp_bytes(uint32_t n_targets, uint32_t n_multi);
 // Largest component the component kernel takes: KB_EM_COMP_CAP (test knob, in the size units above), else unlimited.
 unsigned long long emcomp_cap();
-// Components, slices and the slice bounds; returns stats[0..4] through one device-to-host read.
+// Shared memory the resident layout may take per block: KB_EM_COMP_SMEM (test knob, bytes; 0 keeps the weights
+// streamed), else whatever the device grants a block.
+unsigned long long emcomp_smem_budget();
+// Components, slices and the slice bounds, and the check of the weights against emcomp_weight when w.eff is set;
+// returns stats[0..6] through one device-to-host read.
 void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned long long* stats_host, cudaStream_t st);
-// Per-slice copies of counts, offsets, entries and weights with slice-local 16-bit indices.
-void emcomp_fill(const EmProblem& p, const EmCompWs& w, cudaStream_t st);
+// Per-slice copies of counts, offsets and entries with slice-local 16-bit indices; with `resident`, the effective
+// lengths per pos instead of the weights per entry.
+void emcomp_fill(const EmProblem& p, const EmCompWs& w, bool resident, cudaStream_t st);
 
 // Returns the number of blocks of em_component_kernel it launched, 0 when one of the grid-wide kernels ran.
-// `cw` (optional, one problem): workspace of the component layout.
-int launch_em(const EmProblem& p, int threads_per_block, cudaStream_t st, const EmCompWs* cw = nullptr);
+// `cw` (optional, one problem): workspace of the component layout.  `resident` (optional): set to whether the
+// component kernel held the entries in shared memory.
+int launch_em(const EmProblem& p, int threads_per_block, cudaStream_t st, const EmCompWs* cw = nullptr,
+              bool* resident = nullptr);
 
 // Device-side EM problem construction (kernels_emprep.cu)
 struct EmPrep {

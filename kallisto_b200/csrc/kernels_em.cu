@@ -238,9 +238,13 @@ __global__ void __launch_bounds__(TPB, MINB) em_single_kernel(EmProblem p) {
 }
 
 // One problem whose components fit a block each (kernels.hpp, EmCompWs): every block solves one slice of whole
-// components with its alpha, norm, counts and offsets in shared memory; the entries (16-bit slice-local indices and
-// the weights) stream from the slice's contiguous part of the layout.  Pass A and pass B are em_single_kernel's, statement
-// for statement, with slice-local indices, so every row and every transcript sums exactly what it summed there.
+// components with its alpha, norm, counts and offsets in shared memory.  Streamed (RES = false), the entries (16-bit
+// slice-local indices and the weights) come from the slice's contiguous part of the layout in every round.  Resident
+// (RES = true), the block also holds the entries' indices and the effective lengths (and their reciprocals) of its
+// transcripts, and rebuilds each weight count / eff with emcomp_weight -- the bits calc_weights produced, which
+// emcomp_cut checked for every entry -- so a round touches no global memory.  Pass A and pass B are
+// em_single_kernel's, statement for statement, with slice-local indices, so every row and every transcript sums
+// exactly what it summed there.
 //
 // Components exchange no value, so there is no grid barrier.  Only the stop rule is global (EMAlgorithm.h:170-221):
 // after round i a block adds 1 to sync[2i] if it changed an estimate, then 1 to sync[2i + 1].  A block that changed
@@ -248,7 +252,7 @@ __global__ void __launch_bounds__(TPB, MINB) em_single_kernel(EmProblem p) {
 // until every block has arrived at round i and reads the count.  A block only waits for a round it has reported itself,
 // and all blocks are co-resident (cooperative launch), so no cycle of waits can form.  All blocks see a zero count in
 // the same round, so they evolve the same state and stop after the same round.
-template <int TPB>
+template <int TPB, bool RES>
 __global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCompWs w) {
   extern __shared__ double s_d[];
   __shared__ int s_zero;
@@ -258,20 +262,38 @@ __global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCom
   double* s_alpha = s_d;
   double* s_single = s_alpha + nt;
   double* s_norm = s_single + nt;
-  uint32_t* s_cnt = (uint32_t*)(s_norm + nr);
+  double* s_eff = s_norm + nr;                        // resident: nt each
+  double* s_rcp = s_eff + nt;
+  uint32_t* s_cnt = (uint32_t*)(RES ? s_rcp + nt : s_eff);
   uint32_t* s_roff = s_cnt + nr;          // nr + 1
   uint32_t* s_toff = s_roff + nr + 1;     // nt + 1
+  uint16_t* s_rtid = (uint16_t*)(s_toff + nt + 1);    // resident: the slice's entries, CSR then CSC
+  // resident: offsets relative to the slice's first entry
+  const uint32_t tb = RES ? w.t_off[t0] : 0, rb = RES ? w.r_off[r0] : 0;
   for (uint32_t i = threadIdx.x; i <= nt; i += TPB) {
-    s_toff[i] = w.t_off[t0 + i];
+    s_toff[i] = w.t_off[t0 + i] - tb;
     if (i < nt) {
       s_alpha[i] = p.alpha[w.t_id[t0 + i]];
       s_single[i] = w.t_single[t0 + i];
+      if (RES) {
+        const double e = w.t_eff[t0 + i];
+        s_eff[i] = e;
+        s_rcp[i] = __drcp_rn(e);
+      }
     }
   }
   for (uint32_t k = threadIdx.x; k <= nr; k += TPB) {
-    s_roff[k] = w.r_off[r0 + k];
+    s_roff[k] = w.r_off[r0 + k] - rb;
     if (k < nr) s_cnt[k] = w.r_cnt[r0 + k];
   }
+  const uint32_t ne = RES ? w.r_off[r0 + nr] - rb : 0;
+  uint16_t* s_trow = s_rtid + ne;
+  for (uint32_t j = threadIdx.x; j < ne; j += TPB) {
+    s_rtid[j] = w.r_tid[rb + j];
+    s_trow[j] = w.t_row[tb + j];
+  }
+  const uint16_t* e_tid = RES ? s_rtid : w.r_tid;
+  const uint16_t* e_row = RES ? s_trow : w.t_row;
   __syncthreads();
   const double zero_below = kAlphaLimit / 10.0;
   const bool lead = b == 0 && threadIdx.x == 0;
@@ -284,12 +306,15 @@ __global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCom
       const uint32_t e0 = s_roff[k], e1 = s_roff[k + 1];
       double nrm = 0.0;
       if (c != 0) {
+        const double cd = (double)c;
         double denom = 0.0;
 #pragma unroll 4
         for (uint32_t j = e0; j < e1; ++j) {
-          double a = s_alpha[w.r_tid[j]];
+          const uint32_t t = e_tid[j];
+          double a = s_alpha[t];
           if (fin && a < zero_below) a = 0.0;
-          denom = __dadd_rn(denom, __dmul_rn(a, w.r_w[j]));
+          const double wt = RES ? emcomp_weight(cd, s_eff[t], s_rcp[t]) : w.r_w[j];
+          denom = __dadd_rn(denom, __dmul_rn(a, wt));
         }
         if (!(denom < kTolerance)) nrm = __ddiv_rn((double)c, denom);
       }
@@ -303,9 +328,13 @@ __global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCom
       if (fin && a < zero_below) a = 0.0;
       double acc = s_single[i];
       const uint32_t e0 = s_toff[i], e1 = s_toff[i + 1];
+      const double ef = RES ? s_eff[i] : 0.0, y = RES ? s_rcp[i] : 0.0;
 #pragma unroll 4
-      for (uint32_t j = e0; j < e1; ++j)
-        acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(w.t_w[j], a), s_norm[w.t_row[j]]));
+      for (uint32_t j = e0; j < e1; ++j) {
+        const uint32_t k = e_row[j];
+        const double wt = RES ? emcomp_weight((double)s_cnt[k], ef, y) : w.t_w[j];
+        acc = __dadd_rn(acc, __dmul_rn(__dmul_rn(wt, a), s_norm[k]));
+      }
       changed = changed || (acc > kAlphaChangeLimit && (fabs(__dadd_rn(acc, -a)) / acc) > kAlphaChange);
       s_alpha[i] = acc;
     }
@@ -394,39 +423,51 @@ int em_max_blocks(int tpb, int nb) {
 namespace {
 constexpr int kCompTpb = 1024;
 
-// The component layout and em_component_kernel, when the problem's components fit: returns the blocks launched, or 0
-// (nothing launched) when a component is larger than KB_EM_COMP_CAP, a slice does not fit one block's shared memory
-// or the slices cannot all be resident at once.
-int launch_em_components(const EmProblem& p, const EmCompWs& w, cudaStream_t st) {
-  if (p.n_targets == 0 || p.max_iter < 1 || p.max_iter > w.sync_rounds) return 0;
-  const uint32_t slices = (uint32_t)std::min(device_sm_count(), w.max_slices);
-  unsigned long long s[8];
-  emcomp_cut(p, w, slices, s, st);
-  const unsigned long long n_slices = s[2], smem = s[4];
-  if (s[3] > emcomp_cap()) return 0;
-  const void* fn = (const void*)em_component_kernel<kCompTpb>;
+// Whether n_slices blocks of the component kernel `fn` with `smem` bytes of shared memory each can all be resident.
+bool comp_fits(const void* fn, unsigned long long smem, unsigned long long n_slices) {
   if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::min<unsigned long long>(smem, 1u << 30)) !=
       cudaSuccess) {
     cudaGetLastError();
-    return 0;
+    return false;
   }
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kCompTpb, (size_t)smem) != cudaSuccess) {
     cudaGetLastError();
-    return 0;
+    return false;
   }
-  if ((unsigned long long)per_sm * device_sm_count() < n_slices) return 0;
-  emcomp_fill(p, w, st);
+  return (unsigned long long)per_sm * device_sm_count() >= n_slices;
+}
+
+// The component layout and em_component_kernel, when the problem's components fit: returns the blocks launched, or 0
+// (nothing launched) when a component is larger than KB_EM_COMP_CAP, a slice does not fit one block's shared memory
+// or the slices cannot all be resident at once.  The resident kernel runs when the effective lengths are known, every
+// weight is rebuilt bit for bit and the largest slice's resident layout fits KB_EM_COMP_SMEM and the block; the
+// streamed kernel otherwise.
+int launch_em_components(const EmProblem& p, const EmCompWs& w, cudaStream_t st, bool* resident) {
+  if (p.n_targets == 0 || p.max_iter < 1 || p.max_iter > w.sync_rounds) return 0;
+  const uint32_t slices = (uint32_t)std::min(device_sm_count(), w.max_slices);
+  unsigned long long s[8];
+  emcomp_cut(p, w, slices, s, st);
+  const unsigned long long n_slices = s[2];
+  if (s[3] > emcomp_cap()) return 0;
+  const void* fn_res = (const void*)em_component_kernel<kCompTpb, true>;
+  const bool res = w.eff && s[5] == 0 && s[6] <= emcomp_smem_budget() && comp_fits(fn_res, s[6], n_slices);
+  const void* fn = res ? fn_res : (const void*)em_component_kernel<kCompTpb, false>;
+  const unsigned long long smem = res ? s[6] : s[4];
+  if (!res && !comp_fits(fn, smem, n_slices)) return 0;
+  emcomp_fill(p, w, res, st);
   cudaMemsetAsync(w.sync, 0, 2 * (size_t)p.max_iter * sizeof(unsigned), st);
   EmProblem pp = p;
   EmCompWs ww = w;
   void* args[] = {&pp, &ww};
   cudaLaunchCooperativeKernel(fn, dim3((unsigned)n_slices), dim3(kCompTpb), args, (size_t)smem, st);
+  if (resident) *resident = res;
   return (int)n_slices;
 }
 }  // namespace
 
-int launch_em(const EmProblem& p, int tpb_req, cudaStream_t st, const EmCompWs* cw) {
+int launch_em(const EmProblem& p, int tpb_req, cudaStream_t st, const EmCompWs* cw, bool* resident) {
+  if (resident) *resident = false;
   EmProblem pp = p;
   cudaMemsetAsync(pp.bar, 0, sizeof(unsigned), st);
   {
@@ -439,7 +480,7 @@ int launch_em(const EmProblem& p, int tpb_req, cudaStream_t st, const EmCompWs* 
   if (p.nb == 1 && p.w_stride == 0 && ss.fn) {
     // an explicit KB_EM_SHAPE keeps the grid-wide kernels
     if (cw && !getenv("KB_EM_SHAPE")) {
-      const int blocks = launch_em_components(p, *cw, st);
+      const int blocks = launch_em_components(p, *cw, st, resident);
       if (blocks) return blocks;
     }
     int per_sm = 0;

@@ -310,16 +310,40 @@ __global__ void comp_bounds_kernel(EmProblem p, EmCompWs w) {
   w.s_r0[s] = r0;
   if (s + 1 == n) { w.s_t0[n] = t1; w.s_r0[n] = r1; }
   atomicMax(&w.stats[4], emcomp_smem_bytes(t1 - t0, r1 - r0));
+  // a slice holds whole components, so its size is its transcripts, its rows and its entries
+  const unsigned long long ne = (w.tscan[t1] - w.tscan[t0]) - (t1 - t0) - (r1 - r0);
+  atomicMax(&w.stats[6], emcomp_resident_bytes(t1 - t0, r1 - r0, ne));
+}
+
+// Thread per row and per transcript: counts the entries of the CSR and the CSC whose weight emcomp_weight does not
+// rebuild bit for bit from the row's count and the transcript's effective length.
+__global__ void comp_check_weights_kernel(EmProblem p, EmCompWs w) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long bad = 0;
+  if (i < p.n_multi) {
+    const double c = (double)p.cnt_row[i];
+    for (uint32_t j = p.m_off[i]; j < p.m_off[i + 1]; ++j) {
+      const double e = w.eff[p.m_tid[j]];
+      bad += __double_as_longlong(emcomp_weight(c, e, __drcp_rn(e))) != __double_as_longlong(p.m_w[j]);
+    }
+  }
+  if (i < p.n_targets) {
+    const double e = w.eff[i], y = __drcp_rn(e);
+    for (uint32_t j = p.t_off[i]; j < p.t_off[i + 1]; ++j)
+      bad += __double_as_longlong(emcomp_weight((double)p.cnt_row[p.t_midx[j]], e, y)) != __double_as_longlong(p.t_w[j]);
+  }
+  if (bad) atomicAdd(&w.stats[5], bad);
 }
 
 // Slice-local positions, per-pos counts and entry counts (thread per pos and per row pos).
-__global__ void comp_local_kernel(EmProblem p, EmCompWs w) {
+__global__ void comp_local_kernel(EmProblem p, EmCompWs w, bool resident) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const unsigned long long target = w.stats[1];
   if (i < p.n_targets) {
     const uint32_t t = w.t_id[i];
     w.tloc[t] = i - w.s_t0[w.cstart[w.tkey[i]] / target];
     w.t_single[i] = p.single_cnt[t];
+    if (resident) w.t_eff[i] = w.eff[t];
     w.t_len[i] = p.t_off[t + 1] - p.t_off[t];
   } else if (i == p.n_targets) {
     w.t_len[i] = 0;
@@ -335,14 +359,14 @@ __global__ void comp_local_kernel(EmProblem p, EmCompWs w) {
 }
 
 // Entries in slice order; the order inside a row and inside a transcript's list is kept.
-__global__ void comp_entries_kernel(EmProblem p, EmCompWs w) {
+__global__ void comp_entries_kernel(EmProblem p, EmCompWs w, bool resident) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < p.n_targets) {
     const uint32_t t = w.t_id[i];
     const uint32_t s0 = p.t_off[t], n = p.t_off[t + 1] - s0, d0 = w.t_off[i];
     for (uint32_t j = 0; j < n; ++j) {
       w.t_row[d0 + j] = (uint16_t)w.rloc[p.t_midx[s0 + j]];
-      w.t_w[d0 + j] = p.t_w[s0 + j];
+      if (!resident) w.t_w[d0 + j] = p.t_w[s0 + j];
     }
   }
   if (i < p.n_multi) {
@@ -350,7 +374,7 @@ __global__ void comp_entries_kernel(EmProblem p, EmCompWs w) {
     const uint32_t s0 = p.m_off[r], n = p.m_off[r + 1] - s0, d0 = w.r_off[i];
     for (uint32_t j = 0; j < n; ++j) {
       w.r_tid[d0 + j] = (uint16_t)w.tloc[p.m_tid[s0 + j]];
-      w.r_w[d0 + j] = p.m_w[s0 + j];
+      if (!resident) w.r_w[d0 + j] = p.m_w[s0 + j];
     }
   }
 }
@@ -378,6 +402,11 @@ unsigned long long emcomp_cap() {
   return ~0ull;
 }
 
+unsigned long long emcomp_smem_budget() {
+  if (const char* s = getenv("KB_EM_COMP_SMEM")) return strtoull(s, nullptr, 10);   // test knob
+  return ~0ull;
+}
+
 void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned long long* stats_host, cudaStream_t st) {
   const uint32_t T = p.n_targets, R = p.n_multi;
   const int bits = key_bits(T);
@@ -397,19 +426,20 @@ void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned
   cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.tsize, w.tscan, (int)T + 1, st);
   comp_heads_kernel<<<(T + 255) / 256, 256, 0, st>>>(p, w, slices);
   comp_bounds_kernel<<<(slices + 127) / 128, 128, 0, st>>>(p, w);
+  if (w.eff) comp_check_weights_kernel<<<(std::max(T, R) + 255) / 256, 256, 0, st>>>(p, w);
   cudaMemcpyAsync(stats_host, w.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
   cudaStreamSynchronize(st);
 }
 
-void emcomp_fill(const EmProblem& p, const EmCompWs& w, cudaStream_t st) {
+void emcomp_fill(const EmProblem& p, const EmCompWs& w, bool resident, cudaStream_t st) {
   const uint32_t T = p.n_targets, R = p.n_multi;
   const uint32_t n = std::max(T, R) + 1;
-  comp_local_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w);
+  comp_local_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w, resident);
   size_t tb = w.tmp_bytes;
   cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.t_len, w.t_off, (int)T + 1, st);
   tb = w.tmp_bytes;
   cub::DeviceScan::ExclusiveSum(w.tmp, tb, w.r_len, w.r_off, (int)R + 1, st);
-  comp_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w);
+  comp_entries_kernel<<<(n + 255) / 256, 256, 0, st>>>(p, w, resident);
 }
 
 }  // namespace kb
