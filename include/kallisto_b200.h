@@ -185,6 +185,18 @@ int kb_em_run_table(kb_quant* q, uint32_t n_ecs, const uint64_t* ec_offsets, con
                     const uint32_t* counts, double fld_mean, double fld_sd, double* est_counts_out,
                     double* eff_lens_out, int32_t* rounds_out, double* seconds_out);
 
+/* --priors (EMAlgorithm::read_priors, src/EMAlgorithm.h:52-81).  Host-only.  Reads one value per line with std::stod
+ * (leading blanks skipped, anything after the number ignored) and sums them in file order.  A sum >= 1 + 1e-3 means
+ * raw counts: each value becomes (value + 1) / (sum + n).  Otherwise the values are returned as they are.
+ * Two calls: with out == NULL or cap < n only *n_out is set.  Returns KB_ERR_IO when the file cannot be opened and
+ * KB_ERR_INVALID when a line is not a number std::stod accepts (kb_last_error() names the line). */
+int kb_read_priors(const char* path, double* out, uint64_t cap, uint64_t* n_out);
+/* EMAlgorithm::set_priors (src/EMAlgorithm.h:83-93): every later kb_em_run / kb_em_run_table of q starts from these
+ * n == n_targets values instead of the uniform 1 / n_targets (the values are copied).  Any other n returns
+ * KB_ERR_INVALID and changes nothing; priors == NULL goes back to the uniform start.  kb_bootstrap_run always starts
+ * uniform, as the reference's bootstraps do. */
+int kb_em_set_priors(kb_quant* q, const double* priors, uint32_t n);
+
 /* Replaces the bootstrap loop of main.cpp:2743-2782 (seeds from mt19937_64(seed); per bootstrap
  * Multinomial::sample + Bootstrap::run_em).  est_counts_out is n_bootstrap x n_targets, row-major;
  * samples_out (optional) n_bootstrap x n_ecs resampled counts; rounds_out (optional) n_bootstrap. */
@@ -224,6 +236,13 @@ int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, c
                      const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
                      int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, double* est_counts_out,
                      int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out);
+/* kb_tcc_run_genes with --priors (src/main.cpp:2984-2987,3019): every sample's EM starts from priors (n_targets values)
+ * instead of the uniform 1 / n_targets; priors == NULL is kb_tcc_run_genes.  The bootstrap entry points take no priors:
+ * bootstraps start uniform. */
+int kb_tcc_run_priors(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                      const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                      int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, const double* priors,
+                      double* est_counts_out, int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out);
 typedef int (*kb_tcc_bootstrap_genes_cb)(void* user, uint64_t first, uint32_t count, const double* est_counts,
                                          const int32_t* rounds, const uint32_t* samples, const double* gene_counts,
                                          const double* gene_tpm);

@@ -98,9 +98,9 @@ EXPORTED_SYMBOLS = [
     "kb_index_target_lens", "kb_index_inspect", "kb_quant_create", "kb_quant_free", "kb_pseudoalign_batch",
     "kb_pseudoalign_batch_pe", "kb_host_alloc", "kb_host_free", "kb_pseudoalign_batch_device", "kb_quant_sync", "kb_quant_set_stream", "kb_quant_enable_timing",
     "kb_quant_get_timings", "kb_quant_finalize", "kb_quant_ec_table", "kb_quant_get_flens",
-    "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
+    "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_read_priors", "kb_em_set_priors", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
     "kb_comm_unique_id", "kb_comm_create", "kb_comm_create_from_nccl", "kb_comm_create_all", "kb_comm_reserve", "kb_comm_free",
-    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
+    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_run_priors", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
 ]
 
 # kb_tcc_bootstrap_cb: (user, first problem, count, est_counts, rounds, resampled counts or NULL) -> 0 to go on
@@ -151,6 +151,8 @@ def lib():
     L.kb_quant_set_flens.argtypes = [vp, vp]
     L.kb_em_run.argtypes = [vp, dbl, dbl, vp, vp, C.POINTER(i32), C.POINTER(dbl)]
     L.kb_em_run_table.argtypes = [vp, u32, vp, vp, vp, dbl, dbl, vp, vp, C.POINTER(i32), C.POINTER(dbl)]
+    L.kb_read_priors.argtypes = [C.c_char_p, vp, u64, C.POINTER(u64)]
+    L.kb_em_set_priors.argtypes = [vp, vp, u32]
     L.kb_bootstrap_run.argtypes = [vp, dbl, dbl, u64, i32, vp, vp, vp]
     L.kb_counts_to_tpm.argtypes = [vp, vp, u32, vp]
     L.kb_quant_export_prepare.argtypes = [vp, C.POINTER(u32), C.POINTER(u32)]
@@ -169,6 +171,7 @@ def lib():
     L.kb_tcc_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, vp]
     L.kb_tcc_bootstrap_run.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, u64, i32, i32, TCC_BOOTSTRAP_CB, vp]
     L.kb_tcc_run_genes.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, u32, vp, vp, vp, vp]
+    L.kb_tcc_run_priors.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, u32, vp, vp, vp, vp, vp]
     L.kb_tcc_bootstrap_run_genes.argtypes = [vp, u32, vp, vp, u32, vp, vp, vp, vp, i32, vp, u32, u64, i32, i32,
                                              TCC_BOOTSTRAP_GENES_CB, vp]
     L.kb_eff_lens.argtypes = [vp, vp, dbl, dbl, vp, C.POINTER(dbl), C.POINTER(dbl)]
@@ -198,6 +201,17 @@ def inspect_index(path):
     info = kb_index_info()
     _ck(lib().kb_index_inspect(os.fsencode(path), C.byref(info)))
     return {f: getattr(info, f) for f, _ in kb_index_info._fields_}
+
+
+def read_priors(path):
+    """EMAlgorithm::read_priors (kb_read_priors, host only): the priors of a --priors file as the EM would start from
+    them (raw counts get a pseudocount and are normalised) -> float64 array."""
+    n = C.c_uint64(0)
+    _ck(lib().kb_read_priors(os.fsencode(path), None, 0, C.byref(n)))
+    out = np.zeros(n.value, np.float64)
+    if n.value:
+        _ck(lib().kb_read_priors(os.fsencode(path), _p(out), n.value, C.byref(n)))
+    return out
 
 
 class KmerIndex:
@@ -376,6 +390,15 @@ class MinCollector:
         _ck(lib().kb_quant_reserve(self._h, n_ecs, n_entries))
 
     # -- EMAlgorithm::run / Bootstrap::run_em --------------------------------------------------
+    def set_priors(self, priors):
+        """EMAlgorithm::set_priors: every later run_em starts from `priors` (n_targets values); None goes back to the
+        uniform start.  run_bootstrap always starts uniform."""
+        if priors is None:
+            _ck(lib().kb_em_set_priors(self._h, None, 0))
+            return
+        a = np.ascontiguousarray(priors, np.float64)
+        _ck(lib().kb_em_set_priors(self._h, _p(a), a.size))
+
     def run_em(self, fld_mean=0.0, fld_sd=0.0, table=None):
         T = self.index.num_trans
         est = np.zeros(T, np.float64)
@@ -515,11 +538,12 @@ def _genes_arg(index, genes):
     return gene_of, int(n_genes)
 
 
-def tcc_run(index, ec_sets, rows, eff, genes=None):
+def tcc_run(index, ec_sets, rows, eff, genes=None, priors=None):
     """`kallisto quant-tcc` on the device: ec_sets = list of sorted transcript-id tuples (EC id = position), rows = per sample
     a list of (ec id, count); eff = effective lengths (n_targets, or n_samples x n_targets) -> (est_counts (S, T), rounds (S)).
     genes = (gene of every target, -1 for none; number of genes): gene-level output summed on the device
-    (kb_tcc_run_genes) -> (est_counts, rounds, gene_counts (S, G), gene_tpm (S, G))."""
+    (kb_tcc_run_genes) -> (est_counts, rounds, gene_counts (S, G), gene_tpm (S, G)).  priors (n_targets values): the start of
+    every sample's EM instead of the uniform one (kb_tcc_run_priors)."""
     T = index.num_trans
     eo = np.zeros(len(ec_sets) + 1, np.uint64)
     tids = []
@@ -539,6 +563,19 @@ def tcc_run(index, ec_sets, rows, eff, genes=None):
     per_sample = int(eff.ndim == 2)
     est = np.zeros((len(rows), T), np.float64)
     rounds = np.zeros(max(1, len(rows)), np.int32)
+    if priors is not None:
+        priors = np.ascontiguousarray(priors, np.float64)
+        if priors.shape != (T,):
+            raise ValueError("priors: one value per target (%d), got shape %s" % (T, priors.shape))
+        gene_of, G = _genes_arg(index, genes) if genes is not None else (None, 0)
+        gc = np.zeros((len(rows), max(1, G)), np.float64)
+        gt = np.zeros((len(rows), max(1, G)), np.float64)
+        _ck(lib().kb_tcc_run_priors(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals),
+                                    _p(eff), per_sample, _p(gene_of), G, _p(priors), _p(est), _p(rounds),
+                                    _p(gc) if G else None, _p(gt) if G else None))
+        if genes is None:
+            return est, rounds[: len(rows)]
+        return est, rounds[: len(rows)], gc[:, :G], gt[:, :G]
     if genes is None:
         _ck(lib().kb_tcc_run(index._h, len(ec_sets), _p(eo), _p(tids), len(rows), _p(ro), _p(ids), _p(vals), _p(eff),
                              per_sample, _p(est), _p(rounds)))

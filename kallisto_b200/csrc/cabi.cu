@@ -8,6 +8,7 @@
 #include "../../include/kallisto_b200.h"
 #include "engine.hpp"
 #include "fastx.hpp"
+#include "priors.hpp"
 
 namespace {
 thread_local std::string g_err;
@@ -281,6 +282,27 @@ int kb_em_run_table(kb_quant* q, uint32_t n_ecs, const uint64_t* ec_offsets, con
   });
 }
 
+int kb_read_priors(const char* path, double* out, uint64_t cap, uint64_t* n_out) {
+  if (!path || !n_out) return fail(KB_ERR_INVALID, "kb_read_priors: null argument");
+  std::vector<double> v;
+  uint64_t line = 0;
+  const int r = kb::read_priors_file(path, v, &line);
+  if (r == 1) return fail(KB_ERR_IO, std::string("could not open priors file ") + path);
+  if (r == 2)
+    return fail(KB_ERR_INVALID, "line " + std::to_string(line) + " of priors file " + path + " is not a number");
+  *n_out = v.size();
+  if (out && cap >= v.size() && !v.empty()) memcpy(out, v.data(), v.size() * sizeof(double));
+  return KB_OK;
+}
+
+int kb_em_set_priors(kb_quant* q, const double* priors, uint32_t n) {
+  if (!q) return fail(KB_ERR_INVALID, "kb_em_set_priors: null argument");
+  const uint32_t T = q->q->index().flat.num_targets();
+  if (priors && n != T)
+    return fail(KB_ERR_INVALID, "kb_em_set_priors: " + std::to_string(n) + " priors for " + std::to_string(T) + " targets");
+  return guarded([&] { q->q->set_priors(priors); });
+}
+
 int kb_bootstrap_run(kb_quant* q, double fld_mean, double fld_sd, uint64_t seed, int32_t n_bootstrap,
                      double* est_counts_out, uint32_t* samples_out, int32_t* rounds_out) {
   if (!q || !est_counts_out || n_bootstrap < 0) return fail(KB_ERR_INVALID, "kb_bootstrap_run: bad argument");
@@ -387,10 +409,10 @@ int kb_quant_reserve(kb_quant* q, uint64_t n_ecs, uint64_t n_entries) {
   return guarded([&] { q->q->reserve_em(n_ecs, n_entries); });
 }
 
-int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
-                     const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
-                     int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, double* est_counts_out,
-                     int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out) {
+int kb_tcc_run_priors(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                      const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                      int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, const double* priors,
+                      double* est_counts_out, int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out) {
   if (!ix || !ec_offsets || !row_offsets || !eff_lens || !est_counts_out || (n_ecs && !tids) ||
       (n_genes && (!gene_of_target || !gene_counts_out || !gene_tpm_out)))
     return fail(KB_ERR_INVALID, "kb_tcc_run: null argument");
@@ -398,7 +420,7 @@ int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, c
     kb::TccInput in;
     in.n_ecs = n_ecs; in.ec_off = ec_offsets; in.tids = tids; in.n_samples = n_samples; in.row_off = row_offsets;
     in.ec_ids = ec_ids; in.counts = counts; in.eff_lens = eff_lens; in.per_sample_eff = per_sample_eff != 0;
-    in.gene_of = gene_of_target; in.n_genes = n_genes;
+    in.gene_of = gene_of_target; in.n_genes = n_genes; in.priors = priors;
     std::vector<double> alpha, gc, gt;
     const std::vector<int> rounds = kb::tcc_run(*ix->ix, in, alpha, &gc, &gt);
     memcpy(est_counts_out, alpha.data(), alpha.size() * sizeof(double));
@@ -411,11 +433,19 @@ int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, c
   });
 }
 
+int kb_tcc_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
+                     const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
+                     int32_t per_sample_eff, const int32_t* gene_of_target, uint32_t n_genes, double* est_counts_out,
+                     int32_t* rounds_out, double* gene_counts_out, double* gene_tpm_out) {
+  return kb_tcc_run_priors(ix, n_ecs, ec_offsets, tids, n_samples, row_offsets, ec_ids, counts, eff_lens, per_sample_eff,
+                           gene_of_target, n_genes, nullptr, est_counts_out, rounds_out, gene_counts_out, gene_tpm_out);
+}
+
 int kb_tcc_run(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids, uint32_t n_samples,
                const uint64_t* row_offsets, const uint32_t* ec_ids, const uint32_t* counts, const double* eff_lens,
                int32_t per_sample_eff, double* est_counts_out, int32_t* rounds_out) {
-  return kb_tcc_run_genes(ix, n_ecs, ec_offsets, tids, n_samples, row_offsets, ec_ids, counts, eff_lens, per_sample_eff,
-                          nullptr, 0, est_counts_out, rounds_out, nullptr, nullptr);
+  return kb_tcc_run_priors(ix, n_ecs, ec_offsets, tids, n_samples, row_offsets, ec_ids, counts, eff_lens, per_sample_eff,
+                           nullptr, 0, nullptr, est_counts_out, rounds_out, nullptr, nullptr);
 }
 
 int kb_tcc_bootstrap_run_genes(kb_index* ix, uint32_t n_ecs, const uint64_t* ec_offsets, const uint32_t* tids,

@@ -31,11 +31,14 @@
 
 #include "../../include/kallisto_b200.h"
 // Bound weakly: the command line also links against stand-ins of the library that carry only the entry points of the
-// host pipeline (tests/stub); there `quant-tcc -b` and `quant-tcc -g / -G` report the missing entry point instead of
-// failing to link.
+// host pipeline (tests/stub); there `quant-tcc -b`, `quant-tcc -g / -G` and --priors report the missing entry point
+// instead of failing to link.
 #pragma weak kb_tcc_bootstrap_run
 #pragma weak kb_tcc_run_genes
 #pragma weak kb_tcc_bootstrap_run_genes
+#pragma weak kb_read_priors
+#pragma weak kb_em_set_priors
+#pragma weak kb_tcc_run_priors
 #include "fastx.hpp"
 #include "h5_reader.hpp"
 #include "h5_writer.hpp"
@@ -50,6 +53,30 @@ const char* ERROR_STR = "Error:";   // src/main.cpp:29
 
 void write_index_saved(const std::string& in_path, const std::string& out_path, int k);
 
+// --priors file through kb_read_priors (EMAlgorithm::read_priors, src/EMAlgorithm.h:52-81).  An unreadable file and a line
+// std::stod rejects are errors here; the reference runs uniform on the first and aborts on the second.
+bool read_priors(const std::string& path, std::vector<double>& out) {
+  if (!kb_read_priors) { cerr << "Error: this libkallisto_b200 has no kb_read_priors" << endl; return false; }
+  uint64_t n = 0;
+  int r = kb_read_priors(path.c_str(), nullptr, 0, &n);
+  if (r == KB_OK) {
+    out.resize(n);
+    r = kb_read_priors(path.c_str(), out.data(), n, &n);
+  }
+  if (r != KB_OK) { cerr << ERROR_STR << " " << kb_last_error() << endl; return false; }
+  return true;
+}
+
+// EMAlgorithm::set_priors (src/EMAlgorithm.h:83-93): a count other than the number of targets falls back to the uniform
+// start with two lines on stderr (an empty file silently).  Returns whether the priors apply.
+bool priors_apply(const std::vector<double>& priors, uint32_t n_targets) {
+  if (priors.size() == n_targets) return true;
+  if (!priors.empty())
+    cerr << "[   em] number of priors does not match number of transcripts." << endl
+         << "        defaulting to uniform priors." << endl;
+  return false;
+}
+
 struct Options {
   int threads = 1;
   std::string index, output;
@@ -61,6 +88,7 @@ struct Options {
   int device = 0;
   std::vector<int> devices;   // --devices=0,1,...: reads are dealt to several GPUs, merged over NCCL (csrc/comm.cu)
   std::vector<std::string> files;
+  std::string priors;         // -p / --priors: start of the EM (EMAlgorithm::read_priors / set_priors)
 };
 
 // Outputs are written and flushed: leave without tearing down the CUDA context, the k-mer table and the pinned rings
@@ -112,6 +140,10 @@ void usage_quant() {
             << "-s, --sd=DOUBLE               Estimated standard deviation of fragment length" << endl
             << "                              (default: -l, -s values are estimated from paired" << endl
             << "                               end data, but are required when using --single)" << endl
+            << "-p, --priors                  Priors for the EM algorithm, either as raw counts or as" << endl
+            << "                              probabilities. Pseudocounts are added to raw reads to" << endl
+            << "                              prevent zero valued priors. Supplied in the same order" << endl
+            << "                              as the transcripts in the transcriptome" << endl
             << "-t, --threads=INT             Number of host threads parsing input (default: 1)" << endl
             << "    --device=INT              CUDA device ordinal (default: 0)" << endl
             << "    --devices=LIST            Comma-separated CUDA devices: batches of reads are dealt to all of them," << endl
@@ -124,7 +156,7 @@ void usage_quant() {
 
 void parse_quant(int argc, char** argv, Options& opt) {
   int verbose_flag = 0, plaintext_flag = 0, single_flag = 0, single_overhang_flag = 0, fr = 0, rf = 0, write_index_flag = 0;
-  const char* opt_string = "t:i:l:s:o:b:d:D:";
+  const char* opt_string = "t:i:l:s:o:b:d:D:p:";
   static struct option long_options[] = {
       {"verbose", no_argument, &verbose_flag, 1},
       {"write-index", no_argument, &write_index_flag, 1},
@@ -140,6 +172,7 @@ void parse_quant(int argc, char** argv, Options& opt) {
       {"sd", required_argument, 0, 's'},
       {"output-dir", required_argument, 0, 'o'},
       {"bootstrap-samples", required_argument, 0, 'b'},
+      {"priors", required_argument, 0, 'p'},
       {"device", required_argument, 0, 'D'},
       {"devices", required_argument, 0, 'G'},
       {0, 0, 0, 0}};
@@ -153,6 +186,7 @@ void parse_quant(int argc, char** argv, Options& opt) {
       case 'o': opt.output = optarg; break;
       case 'b': std::stringstream(optarg) >> opt.bootstrap; break;
       case 'd': std::stringstream(optarg) >> opt.seed; break;
+      case 'p': opt.priors = optarg; break;
       case 'D': std::stringstream(optarg) >> opt.device; break;
       case 'G': {
         std::stringstream ss(optarg);
@@ -607,6 +641,9 @@ int cmd_quant(int argc, char** argv, const std::string& call, const std::string&
     usage_quant();
     return 1;
   }
+  // read before any device work, so that a bad file stops the run at once
+  std::vector<double> priors;
+  if (!opt.priors.empty() && !read_priors(opt.priors, priors)) return 1;
   PhaseTimer pt;
   // The driver initialises every VISIBLE GPU when the first CUDA call is made (about 0.1 s apiece on an 8-GPU node):
   // unless the caller set CUDA_VISIBLE_DEVICES already, only the devices this run uses are made visible.
@@ -766,6 +803,15 @@ int cmd_quant(int argc, char** argv, const std::string& call, const std::string&
       // MinCollector::get_mean_frag_len (src/MinCollector.cpp:583-607) would stop here as well
     }
   }
+  // the run that solves the EM (the root with --devices) starts from the priors (src/main.cpp:2683-2689)
+  std::string priors_msg;
+  if (!opt.priors.empty()) {
+    priors_msg = "[   em] reading priors from file " + opt.priors + "\n";
+    if (priors.size() == T) {
+      if (!kb_em_set_priors) { cerr << "Error: this libkallisto_b200 has no kb_em_set_priors" << endl; return 1; }
+      KB_TRY(kb_em_set_priors(q, priors.data(), T));
+    }
+  }
   KB_TRY(kb_em_run(q, opt.fld, opt.sd, est.data(), eff.data(), &rounds, nullptr));
   pt.mark("EM");
   if (pt.on) {
@@ -785,6 +831,10 @@ int cmd_quant(int argc, char** argv, const std::string& call, const std::string&
     uint64_t cnt = 0;
     for (size_t i = 0; i < 1000; ++i) { mass += (double)(flens[i] * i); cnt += flens[i]; }
     cerr << "[quant] estimated average fragment length: " << (cnt ? mass / (double)cnt : 0.0) << endl;
+  }
+  if (!opt.priors.empty()) {
+    cerr << priors_msg;
+    priors_apply(priors, T);
   }
   cerr << "[   em] quantifying the abundances ... done" << endl;
   cerr << "[   em] the Expectation-Maximization algorithm ran for " << pretty_num((size_t)rounds) << " rounds" << endl;
@@ -1393,12 +1443,16 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
 // equivalence classes of the EC file; all rows are solved on the device by the batched EM kernel (kb_tcc_run), and
 // their bootstraps (-b) likewise, every (row, bootstrap) pair its own problem (kb_tcc_bootstrap_run).
 // Supported: -i, -e (required here), -o, -l/-s, -f, -t, -b, -d/--seed, -g/--genemap, -G/--gtf, --matrix-to-files,
-// --matrix-to-directories, --plaintext.  Gene-level output is summed on the device (kb_tcc_run_genes,
-// kb_tcc_bootstrap_run_genes).  Priors, --long, -T and a per-sample abundance.h5 are refused loudly.
+// --matrix-to-directories, --plaintext, -p/--priors.  Gene-level output is summed on the device (kb_tcc_run_genes,
+// kb_tcc_bootstrap_run_genes).  Priors start every sample's EM (kb_tcc_run_priors); bootstraps start uniform, as in the
+// reference.  --long, -T and a per-sample abundance.h5 are refused loudly.
 // Deliberate differences from the reference:
 //   - -b on a matrix file without --matrix-to-files / --matrix-to-directories, or without --plaintext, is refused: the
 //     reference (built without HDF5) runs and silently writes no bootstraps there.
 //   - -b on a non-matrix file whose counts are all zero is an error; the reference aborts (Multinomial::sample(0)).
+//   - --priors (here and in quant): a file that cannot be opened is an error ("Error: could not open priors file
+//     <path>", exit 1); the reference silently starts uniform.  A line std::stod rejects (an empty line, `abc`, `1e999`)
+//     is an error naming the line, exit 1; the reference aborts with an uncaught exception.
 // ------------------------------------------------------------------------------------------------
 void usage_tcc() {
   std::cout << "kallisto_b200 " << KALLISTO_VERSION << " (H100 build)" << endl
@@ -1413,6 +1467,10 @@ void usage_tcc() {
             << "                              (default: effective length normalization is not performed)" << endl
             << "-l, --fragment-length=DOUBLE  Estimated average fragment length" << endl
             << "-s, --sd=DOUBLE               Estimated standard deviation of fragment length" << endl
+            << "-p, --priors                  Priors for the EM algorithm, either as raw counts or as" << endl
+            << "                              probabilities. Pseudocounts are added to raw reads to" << endl
+            << "                              prevent zero valued priors. Supplied in the same order" << endl
+            << "                              as the transcripts in the transcriptome" << endl
             << "-t, --threads=INT             Number of host threads (default: 1)" << endl
             << "-b, --bootstrap-samples=INT   Number of bootstrap samples (default: 0); with a matrix file only" << endl
             << "                              together with --matrix-to-files or --matrix-to-directories and --plaintext" << endl
@@ -1711,7 +1769,7 @@ int cmd_quant_tcc(int argc, char** argv) {
   if (!genemap.empty() && !gtf.empty()) { cerr << ERROR_STR << " Cannot supply both --genemap and --gtf" << endl; ret = false; }
   if (!gtf.empty() && stat(gtf.c_str(), &stt) != 0) { cerr << ERROR_STR << " GTF file not found " << gtf << endl; ret = false; }
   if (!genemap.empty() && stat(genemap.c_str(), &stt) != 0) { cerr << ERROR_STR << " file for mapping transcripts to genes not found " << genemap << endl; ret = false; }
-  if (!priors.empty() || long_flag || !txnames.empty()) { cerr << ERROR_STR << " --priors, --long and --txnames are not supported by this build" << endl; ret = false; }
+  if (long_flag || !txnames.empty()) { cerr << ERROR_STR << " --long and --txnames are not supported by this build" << endl; ret = false; }
   if (bootstrap > 0 && (!matrix_to_files || !plaintext) && !tccfile.empty()) {
     std::ifstream in(tccfile);
     std::string first;
@@ -1733,6 +1791,9 @@ int cmd_quant_tcc(int argc, char** argv) {
   if (threads <= 0) { cerr << ERROR_STR << " invalid number of threads " << threads << endl; ret = false; }
   if (bootstrap < 0) { cerr << "Error: number of bootstrap samples must be a non-negative integer." << endl; ret = false; }
   if (!ret) { cerr << endl; usage_tcc(); return 1; }
+  // the priors file is read once, before any device work (src/main.cpp:2984-2987)
+  std::vector<double> prior_v;
+  if (!priors.empty() && !read_priors(priors, prior_v)) return 1;
 
   kb_index* ix = nullptr;
   KB_TRY(kb_index_load(index.c_str(), device, 0, std::min(16, std::max(1, threads)), &ix));
@@ -1899,7 +1960,20 @@ int cmd_quant_tcc(int argc, char** argv) {
   cerr << "[quant] Running EM algorithm..." << endl;
   std::vector<double> est(nrow * (size_t)T), gene_counts(gene_level ? nrow * (size_t)G : 0), gene_tpm(gene_counts.size());
   std::vector<int32_t> rounds(nrow + 1);
-  if (gene_level) {
+  // every sample's EM starts from the priors (src/main.cpp:3019): a count mismatch is reported once per sample
+  bool use_priors = false;
+  if (!priors.empty()) {
+    cerr << "[   em] reading priors from file " << priors << endl;
+    for (size_t r = 0; r < nrow; ++r) use_priors = priors_apply(prior_v, T);
+  }
+  if (use_priors) {
+    if (!kb_tcc_run_priors) { cerr << "Error: this libkallisto_b200 has no kb_tcc_run_priors" << endl; return 1; }
+    KB_TRY(kb_tcc_run_priors(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow,
+                             row_off.data(), ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(),
+                             eff.data(), per_sample ? 1 : 0, gene_level ? gm.gene_of.data() : nullptr, G, prior_v.data(),
+                             est.data(), rounds.data(), gene_level ? gene_counts.data() : nullptr,
+                             gene_level ? gene_tpm.data() : nullptr));
+  } else if (gene_level) {
     if (!kb_tcc_run_genes) { cerr << "Error: this libkallisto_b200 has no kb_tcc_run_genes" << endl; return 1; }
     KB_TRY(kb_tcc_run_genes(ix, n_ecs, ec_off.data(), ec_tids.empty() ? nullptr : ec_tids.data(), (uint32_t)nrow,
                             row_off.data(), ids.empty() ? nullptr : ids.data(), vals.empty() ? nullptr : vals.data(),

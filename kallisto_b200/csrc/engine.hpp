@@ -56,8 +56,10 @@ struct BatchWs {
 };
 
 // The per-problem device state of launch_em for up to `cap` problems (grow-only), and the one host-side driver of every
-// EM batch: launch() starts the problems from a uniform alpha with zeroed round counts, final states and change
-// counters; fetch() downloads their estimates and round counts and applies the state-3 zeroing.
+// EM batch: launch() starts the problems from the given priors (or a uniform alpha) with zeroed round counts, final
+// states and change counters; fetch() downloads their estimates and round counts and applies the state-3 zeroing.
+// Bootstraps always start uniform (Bootstrap::run_em builds a fresh EMAlgorithm, src/Bootstrap.cpp:4-13): their
+// callers pass no priors.
 struct EmState {
   DBuf<double> alpha, norm, single_cnt;
   DBuf<uint32_t> cnt_row;
@@ -67,9 +69,11 @@ struct EmState {
   size_t cap = 0;
   void reserve(size_t nb, uint32_t T, size_t n_multi);
   // p: the shared structure filled in by the caller (n_ec .. w_set, max_iter, min_rounds); its per-problem fields are
-  // pointed at this state.  `start` (optional) is recorded right before launch_em.  Returns what launch_em returns.
+  // pointed at this state.  `start` (optional) is recorded right before launch_em.  `prior` (optional, device, n_targets
+  // doubles): the start of every problem instead of the uniform 1 / n_targets.  Returns what launch_em returns.
   int launch(EmProblem& p, int nb, const uint32_t* counts, int threads_per_block, cudaStream_t st,
-             const EmCompWs* cw = nullptr, cudaEvent_t start = nullptr, bool* comp_resident = nullptr);
+             const EmCompWs* cw = nullptr, cudaEvent_t start = nullptr, bool* comp_resident = nullptr,
+             const double* prior = nullptr);
   // Enqueues the download of p's nb x n_targets estimates and nb rounds behind whatever the caller enqueued since
   // launch(), synchronises the stream once and zeroes the small estimates of problems that stopped in state 3.
   void fetch(const EmProblem& p, double* alpha_out, int* rounds_out, cudaStream_t st);
@@ -265,6 +269,11 @@ class Quant {
   // Size the EM / EC-numbering workspace ahead of time (no cudaMalloc on the first kb_em_run).
   void reserve_em(size_t n_ecs, size_t n_entries);
 
+  // --priors (EMAlgorithm::set_priors, src/EMAlgorithm.h:83-93): n_targets start values of every later run_em /
+  // run_em_device, uploaded once; nullptr goes back to the uniform start.  Bootstraps ignore them.
+  void set_priors(const double* priors);
+  bool has_priors() const { return has_priors_; }
+
   // Same result on the EM matrices run_em_device left on the device (no EC table on the host, no second set-up);
   // the B problems are solved `chunk` at a time so that their alpha / norm vectors stay in L2.  ms_out (optional):
   // {resample ms, EM ms} measured with CUDA events.
@@ -333,6 +342,8 @@ class Quant {
   std::vector<uint16_t> h_tl_;
   EcTable ecs_;
   bool ecs_valid_ = false;
+  DBuf<double> priors_;
+  bool has_priors_ = false;
   struct EmWs* emws_ = nullptr;
   // bus mode
   DBuf<uint8_t> bus_b_[4], bus_skip_, bus_notag_;
@@ -369,6 +380,9 @@ struct TccInput {
   // computed and nothing for it is allocated.
   const int32_t* gene_of = nullptr;
   uint32_t n_genes = 0;
+  // --priors: the start of every sample's EM (n_targets values, host), nullptr for the uniform start.  tcc_bootstrap
+  // ignores it: bootstraps start uniform, as the reference's do.
+  const double* priors = nullptr;
 };
 // gene_counts_out / gene_tpm_out (n_samples x n_genes) are filled when in.n_genes > 0.
 std::vector<int> tcc_run(Index& ix, const TccInput& in, std::vector<double>& alpha_out /* n_samples x n_targets */,

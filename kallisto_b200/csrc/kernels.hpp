@@ -88,7 +88,6 @@ struct ResolveArgs {
 
 void launch_fill_u64(unsigned long long* p, uint64_t n, unsigned long long v, cudaStream_t st);
 void launch_fill_i32(int32_t* p, uint64_t n, int32_t v, cudaStream_t st);
-void launch_fill_f64(double* p, uint64_t n, double v, cudaStream_t st);
 void launch_fill_memo2(Memo2Entry* p, uint64_t n, cudaStream_t st);
 void launch_build_table(const TableBuildArgs& a, cudaStream_t st);
 void launch_dict_init(const DictInitArgs& a, cudaStream_t st);
@@ -245,6 +244,10 @@ void emcomp_cut(const EmProblem& p, const EmCompWs& w, uint32_t slices, unsigned
 // Per-slice copies of counts, offsets and entries with slice-local 16-bit indices; with `resident`, the effective
 // lengths per pos instead of the weights per entry.
 void emcomp_fill(const EmProblem& p, const EmCompWs& w, bool resident, cudaStream_t st);
+
+// The start state of nb problems over T targets, alpha[b * T + t]: prior[t] when `prior` (T doubles, device) is given,
+// else `uniform` (the caller's 1.0 / T, EMAlgorithm.h:38).
+void launch_em_start(double* alpha, uint32_t nb, uint32_t T, const double* prior, double uniform, cudaStream_t st);
 
 // Returns the number of blocks of em_component_kernel it launched, 0 when one of the grid-wide kernels ran.
 // `cw` (optional, one problem): workspace of the component layout.  `resident` (optional): set to whether the

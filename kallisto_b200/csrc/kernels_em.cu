@@ -369,6 +369,20 @@ __global__ void __launch_bounds__(TPB, 1) em_component_kernel(EmProblem p, EmCom
   for (uint32_t i = threadIdx.x; i < nt; i += TPB) p.alpha[w.t_id[t0 + i]] = s_alpha[i];
 }
 
+// Start state of every problem of a launch: the caller's priors broadcast to each problem (EMAlgorithm::set_priors,
+// EMAlgorithm.h:83-93), or the uniform 1 / T.
+__global__ void em_start_kernel(double* alpha, uint32_t nb, uint32_t T, const double* prior, double uniform) {
+  for (uint32_t b = blockIdx.y; b < nb; b += gridDim.y)
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < T; t += gridDim.x * blockDim.x)
+      alpha[(size_t)b * T + t] = prior ? prior[t] : uniform;
+}
+void launch_em_start(double* alpha, uint32_t nb, uint32_t T, const double* prior, double uniform, cudaStream_t st) {
+  if (nb == 0 || T == 0) return;
+  const unsigned gx = (unsigned)std::min<uint32_t>(256, (T + 255) / 256);
+  const unsigned gy = std::min<uint32_t>(nb, 65535);
+  em_start_kernel<<<dim3(gx, gy), 256, 0, st>>>(alpha, nb, T, prior, uniform);
+}
+
 // Row-ordered copies of the counts the passes need: cnt_row[b][r] = counts[b][multi_ec[r]],
 // single_cnt[b][t] = counts[b][t_single[t]] (as a double) or 0.
 __global__ void em_gather_counts_kernel(EmProblem p) {

@@ -98,10 +98,6 @@ __global__ void fill_i32_kernel(int32_t* p, uint64_t n, int32_t v) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
 }
-__global__ void fill_f64_kernel(double* p, uint64_t n, double v) {
-  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) p[i] = v;
-}
 __global__ void fill_slots_kernel(KmerSlot* p, uint64_t n) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
@@ -122,10 +118,6 @@ void launch_fill_memo2(Memo2Entry* p, uint64_t n, cudaStream_t st) {
 void launch_fill_i32(int32_t* p, uint64_t n, int32_t v, cudaStream_t st) {
   if (n == 0) return;
   fill_i32_kernel<<<device_sm_count() * 8, 256, 0, st>>>(p, n, v);
-}
-void launch_fill_f64(double* p, uint64_t n, double v, cudaStream_t st) {
-  if (n == 0) return;
-  fill_f64_kernel<<<device_sm_count() * 8, 256, 0, st>>>(p, n, v);
 }
 void launch_build_table(const TableBuildArgs& a, cudaStream_t st) {
   fill_slots_kernel<<<device_sm_count() * 8, 256, 0, st>>>(a.slots, a.mask + 1);
