@@ -176,6 +176,8 @@ std::unique_ptr<Index> Index::load(const std::string& path, int device, bool loa
   }
   if (const char* s = getenv("KB_TABLE_FACTOR")) { const double v = atof(s); if (v >= 1.25 && v <= 64.0) factor = v; }
   ix->table_cap = pow2_ge(std::max<uint64_t>(1024, (uint64_t)((double)f.n_kmers * factor)));
+  // match_kernel keeps a probe's slot index in 32 bits (128 GB of slots)
+  if (ix->table_cap > (1ull << 32)) throw Error("kallisto_b200: k-mer table larger than 2^32 slots");
   ix->slots.alloc(ix->table_cap);
   // presence filter: 2^KB_FILTER_LOG2 bits (default: about 3.5 bits per k-mer, at most 2^28 bits = 32 MB so that it
   // fits the persisting part of the H100's 50 MB L2; 0 = off).  Single hash: a miss passes it with probability

@@ -74,9 +74,11 @@ static constexpr int KB_Q_STRIDE = 2 + KB_MAX_E + 6;   // frag, n|flags, handles
 static constexpr int KB_SPILL = 112;                   // a fragment may hit KB_MAX_E + KB_SPILL = 128 distinct EC sets
 static constexpr int KB_QBIG_STRIDE = 2 + KB_MAX_E + KB_SPILL + 6;
 static constexpr uint32_t KB_QBIG_CAP = 1u << 16;      // wide-queue entries per batch
-// match_kernel's shared memory per lane, in 32-bit words: the handle tuple, 6 words per lookup chain (first hit, the
-// reference's nextPos, the second hit of a jump), then the 2-bit bases of both mates (2 x 2 nb words)
-static constexpr int KB_CHAIN_WORDS = 6;
+// match_kernel's shared memory per lane, in 32-bit words: the handle tuple, 11 words per lookup chain (first hit, the
+// reference's nextPos, the second hit of a jump, the jump and middle positions, the distance to the end of the EC block
+// and the anchor hit of a jump), then the 2-bit bases of both mates (2 x 2 nb words).  At 2 x 100 bp (nb = 4) that is
+// 54 words = 216 B per lane, so four blocks of 256 lanes (55.3 KB each + 1 KB reserved per block) fit in an SM's 228 KB
+static constexpr int KB_CHAIN_WORDS = 11;
 __host__ __device__ constexpr size_t match_lane_words(uint32_t nb) { return (size_t)KB_MAX_E + 2 * KB_CHAIN_WORDS + 4 * (size_t)nb; }
 
 struct ResolveArgs {

@@ -21,11 +21,10 @@
 #include "kernels.hpp"
 
 #ifndef KB_MATCH_MIN_BLOCKS
-// 3 blocks of 256 lanes per SM (1 536 lanes, two lookup chains each) at up to 80 registers: at 4 blocks the two chains'
-// state no longer fits in 64 registers and the spills in the lookup loop cost more than the extra lanes gain
+// 3 blocks of 256 lanes per SM (1 536 lanes, two lookup chains each) at up to 80 registers, with no local memory; at 4
+// blocks the 64 registers still do not hold the two chains' state and the lookup loop spills
 #define KB_MATCH_MIN_BLOCKS 3
 #endif
-
 #ifdef KB_MATCH_STATS
 #include <cstdio>
 #endif
@@ -39,13 +38,16 @@ enum : int {
   MS_WARP_ITERS, MS_SERVICE_ROUNDS, MS_LANE_ITERS, MS_CHAIN_ITERS,
   MS_MAIN_HIT, MS_MAIN_MISS_FILTER, MS_MAIN_MISS_SLOT, MS_JUMP, MS_MIDDLE, MS_BACKOFF, MS_COLLISION,
   MS_CYCLES_LOOKUP, MS_CYCLES_SERVICE,
+  // split of a lane-iteration's cycles, summed over lanes (cycles_lookup and cycles_service are lane 0's): keys and hashes
+  // up to the filter loads, the wait for the filter and slot loads, and the state transitions (with the handle dedup)
+  MS_CYCLES_KEY, MS_CYCLES_WAIT, MS_CYCLES_STEP,
   MS_RUN_HIST, MS_N = MS_RUN_HIST + 9     // MAIN miss runs of 1, 2, 3, 4, 5-8, 9-16, 17-32, 33-64, 65+ positions
 };
 __device__ unsigned long long kb_match_stats[MS_N];
 static const char* const kMatchStatNames[MS_N] = {
   "warp_iters", "service_rounds", "lane_iters", "chain_iters",
   "main_hit", "main_miss_filter", "main_miss_slot", "jump", "middle", "backoff", "collision",
-  "cycles_lookup", "cycles_service",
+  "cycles_lookup", "cycles_service", "cycles_key", "cycles_wait", "cycles_step",
   "run_1", "run_2", "run_3", "run_4", "run_5_8", "run_9_16", "run_17_32", "run_33_64", "run_65_"};
 __device__ __forceinline__ int run_bin(int n) {
   return n <= 4 ? n - 1 : (n <= 8 ? 4 : (n <= 16 ? 5 : (n <= 32 ? 6 : (n <= 64 ? 7 : 8))));
@@ -186,8 +188,12 @@ enum : int {
   S_EMPTY = 5                                            // no fragment assigned
 };
 // Cold words of a chain in shared memory: word w of chain c of a lane is its per-lane word KB_MAX_E + 2 * w + c.  The
-// first three (the chain's first hit) are overwritten when a finalised tuple grows past KB_MAX_E.
-enum : int { C_BLK = 0, C_DS = 1, C_POS = 2, C_NP = 3, C_H2U = 4, C_H2E = 5 };
+// first three (the chain's first hit) are overwritten when a finalised tuple grows past KB_MAX_E.  The rest are only
+// read when a JUMP or MIDDLE key is formed and in the transitions out of those states: the reference's nextPos, the
+// second hit of a jump (unitig, set handle), the jump and middle positions, the distance to the end of the EC block and
+// the hit the jump started from (unitig, set handle).
+enum : int { C_BLK = 0, C_DS = 1, C_POS = 2, C_NP = 3, C_H2U = 4, C_H2E = 5, C_P2 = 6, C_P3 = 7, C_DIST = 8, C_HU = 9, C_HE = 10 };
+static_assert(C_HE + 1 == KB_CHAIN_WORDS, "match_lane_words counts every cold word of a chain");
 
 }  // namespace
 
@@ -350,7 +356,8 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
   uint32_t* cold = elist + (size_t)KB_MAX_E * nt;                // [2 * KB_CHAIN_WORDS]
   uint32_t* s_bw = cold + (size_t)2 * KB_CHAIN_WORDS * nt;       // [mate][nw]
   uint32_t* spill = ba.spill + ((size_t)blockIdx.x * nt + tid) * KB_SPILL;   // handles beyond KB_MAX_E (global memory)
-  static_assert(C_BLK < C_POS && C_DS < C_POS && C_POS == 2 && C_NP > C_POS && C_H2U > C_POS && C_H2E > C_POS,
+  // the cold words after the first hit (C_NP .. C_HE) are in enum order
+  static_assert(C_BLK < C_POS && C_DS < C_POS && C_POS == 2 && C_NP == C_POS + 1 && C_HE == KB_CHAIN_WORDS - 1,
                 "a tuple grown by 6 words past KB_MAX_E overwrites exactly the first-hit words of both chains");
   auto cw = [&](int w, int c) -> uint32_t& { return cold[(size_t)(2 * w + c) * nt]; };
 
@@ -363,24 +370,30 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
   const int n_mates = ba.paired ? 2 : 1;
   const int n_chunks = (int)(ba.pstride >> 3);   // 32-byte pieces per packed read
 
+  // the block's totals of lookups, slot visits and memo hits, added to by each warp's service rounds
+  __shared__ unsigned long long s_tot[3];
+  if (tid < 3) s_tot[tid] = 0;
+  __syncthreads();
+
   // per fragment
   uint32_t frag = 0;
   int n_e = 0;
   bool overflow = false;
   unsigned inv_flags = 0;    // bit m: mate m holds a base other than A/C/G/T
-  // per chain (index = mate); np (the reference's nextPos), the second hit of a jump and the first hit live in `cold`
+  // per chain (index = mate); the state of a jump or middle probe and the first hit live in `cold`
   int st[2] = {S_EMPTY, S_EMPTY};
-  int p[2] = {-1, -1}, p2[2] = {-1, -1}, p3[2] = {-1, -1}, dist[2] = {0, 0}, len[2] = {0, 0};
-  uint32_t hu[2] = {0, 0}, he[2] = {0, 0};
+  int p[2] = {-1, -1}, len[2] = {0, 0};
   bool need_prep[2] = {false, false}, is_canon[2] = {false, false};
   bool hv[2] = {false, false}, hs[2] = {false, false};   // the mate has a hit / a hit on a non-empty EC set
-  uint64_t canon[2] = {0, 0}, slot[2] = {0, 0};
-  uint32_t n_probes = 0, n_visits = 0, n_memo = 0;   // per-lane totals: touched once per fragment (they live in local memory)
-  uint32_t pv = 0;          // hot-loop counter of the current fragment: lookups in the low half, slot visits in the high half
+  uint64_t canon[2] = {0, 0};
+  uint32_t slot[2] = {0, 0};   // the table has at most 2^32 slots (KmerIndex load)
+  const uint32_t slot_mask = (uint32_t)ix.mask;
+  uint32_t pv = 0;          // counter of the current fragment: lookups in the low half, slot visits in the high half
 #ifdef KB_MATCH_STATS
   unsigned long long ms[MS_N] = {};
   int run[2] = {0, 0};      // current MAIN miss run of each chain, in positions
   long long t_mark = clock64();
+  long long t_step = -1;    // >= 0: the lane's state transitions of this lookup iteration started at this clock
   auto end_run = [&](int c) { if (run[c] > 0) { KB_MS(MS_RUN_HIST + run_bin(run[c]), 1); run[c] = 0; } };
 #endif
   // view of mate c of the lane's fragment
@@ -402,7 +415,9 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     {
       const long long t_now = clock64();
       KB_MS(in_service ? MS_CYCLES_SERVICE : MS_CYCLES_LOOKUP, t_now - t_mark);
+      if (t_step >= 0) KB_MS(MS_CYCLES_STEP, t_now - t_step);
       t_mark = t_now;
+      t_step = -1;
     }
 #endif
     // ------------------------------------------------------------------ service round
@@ -416,9 +431,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
       KB_MS(MS_SERVICE_ROUNDS, 1);
       KB_MS_ONLY(in_service = true;)
       if (done) {
-        n_probes += pv & 0xFFFFu;     // a fragment executes at most a few hundred lookups
-        n_visits += pv >> 16;
-        pv = 0;
+        bool memo_hit = false;
         // ---- MinCollector::intersectKmers, net effect (MinCollector.cpp:160-218) ----
         const bool v0 = hv[0], s0 = hs[0], v1 = hv[1], s1 = hs[1];
         // first hit of each mate, before the tuple may grow over it
@@ -445,11 +458,12 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             // ProcessReads.cpp:1526): "no first hit" for both mates makes resolve_kernel skip the filter
             if (ba.notag && ba.notag[frag]) xs0 = xs1 = 0xFFFFFFFFu;
           }
-          const int xc = v1 ? 1 : 0;       // the second mate's first hit; the first mate's when the second has none
-          const uint32_t xf0 = f_blk[xc];
-          const uint32_t xf1 = f_ds[xc] >> 31;
-          const uint32_t xf2 = f_pos[xc];
-          const uint32_t xf3 = f_ds[xc] & 0x7FFFFFFFu;
+          // the second mate's first hit; the first mate's when the second has none
+          const uint32_t x_blk = v1 ? f_blk[1] : f_blk[0], x_ds = v1 ? f_ds[1] : f_ds[0], x_pos = v1 ? f_pos[1] : f_pos[0];
+          const uint32_t xf0 = x_blk;
+          const uint32_t xf1 = x_ds >> 31;
+          const uint32_t xf2 = x_pos;
+          const uint32_t xf3 = x_ds & 0x7FFFFFFFu;
           const int nx = (stranded ? 2 : 0) + (want_fp ? 4 : 0);
           // appends the extra words to a tuple stored with stride `st` starting at index `at`
           auto put_extras = [&](uint32_t* dst, int at, int st) {
@@ -509,7 +523,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
                 for (int i = 0; i < n; ++i) e[2 + i] = elist[i * nt];
               } else {
                 handle = r;
-                ++n_memo;
+                memo_hit = true;
               }
             }
           }
@@ -543,6 +557,15 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
         if (handle >= 0 && lane == (unsigned)(__ffs(grp) - 1)) {
           atomicAdd(&dd.count[handle], (uint32_t)__popc(grp));
           atomicMin(&dd.first[handle], (unsigned long long)(ba.frag_base + fmin));
+        }
+        // statistics of the round's fragments (a fragment executes at most a few hundred lookups)
+        const uint32_t r_probes = __reduce_add_sync(fin, pv & 0xFFFFu), r_visits = __reduce_add_sync(fin, pv >> 16);
+        const uint32_t r_memo = __popc(__ballot_sync(fin, memo_hit));
+        pv = 0;
+        if (lane == (unsigned)(__ffs(fin) - 1)) {
+          atomicAdd(&s_tot[0], (unsigned long long)r_probes);
+          atomicAdd(&s_tot[1], (unsigned long long)r_visits);
+          if (r_memo) atomicAdd(&s_tot[2], (unsigned long long)r_memo);
         }
         st[0] = st[1] = S_EMPTY;
       }
@@ -619,25 +642,29 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         if (live[c] && need_prep[c]) {
-          const int pq = (st[c] == S_JUMP) ? p2[c] : ((st[c] == S_MIDDLE) ? p3[c] : p[c]);
+          const bool filtered = st[c] == S_MAIN || st[c] == S_BACKOFF;
+          const int pq = filtered ? p[c] : (int)cw(st[c] == S_JUMP ? C_P2 : C_P3, c);
           const uint64_t fwd = view(c).kmer(pq);
           const uint64_t rc = kb_revcomp(fwd, k);
           is_canon[c] = fwd < rc;
           canon[c] = is_canon[c] ? fwd : rc;
           const uint64_t hsh = kb_mix64(canon[c]);
-          slot[c] = hsh & ix.mask;
+          slot[c] = (uint32_t)hsh & slot_mask;
           need_prep[c] = false;
           ++pv;
           // a clear bit means the k-mer is not in the index -- no HBM sector is touched.  The jump target and the
           // middle k-mer lie in the EC block of the hit before them and are nearly always present: their slot is
           // loaded without the filter word, which would only add an L2 round trip and an L2 request
-          if (ix.filter && (st[c] == S_MAIN || st[c] == S_BACKOFF)) {
+          if (ix.filter && filtered) {
             const uint32_t fidx = (uint32_t)(hsh >> 32) & ix.filter_mask;
             fword[c] = __ldg(ix.filter + (fidx >> 5));
             fbit[c] = fidx & 31;
           }
         }
       }
+#ifdef KB_MATCH_STATS
+      const long long t_key = clock64();
+#endif
       // both slot loads before either is used
       uint32_t v[2][8];
 #pragma unroll
@@ -649,13 +676,25 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
           v[c][0] = v[c][1] = 0xFFFFFFFFu;     // reads as an empty slot: a miss
         }
       }
+#ifdef KB_MATCH_STATS
+      {
+        // the clock is read once both slots (and so both filter words) have arrived: the read is under a branch on the
+        // loaded words, and a volatile read cannot be hoisted above it (the untaken side, a key pair that spells
+        // 0x0BADF00D, only loses that iteration's wait)
+        long long t_wait = t_key;
+        if (((v[0][0] ^ v[0][1]) ^ 3u * (v[1][0] ^ v[1][1])) != 0x0BADF00Du) t_wait = clock64();
+        KB_MS(MS_CYCLES_KEY, t_key - t_mark);
+        KB_MS(MS_CYCLES_WAIT, t_wait - t_key);
+        t_step = t_wait;
+      }
+#endif
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         if (!live[c]) continue;
         KB_MS(MS_CHAIN_ITERS, 1);
         const uint64_t key = (uint64_t)v[c][0] | ((uint64_t)v[c][1] << 32);
         if (key != canon[c] && key != KB_EMPTY_KEY) {
-          slot[c] = (slot[c] + 1) & ix.mask;        // linear probing: one more iteration
+          slot[c] = (slot[c] + 1) & slot_mask;      // linear probing: one more iteration
           KB_MS(MS_COLLISION, 1);
           continue;
         }
@@ -682,15 +721,17 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             push = true;
             const int r_dist = (int)(v[c][5] & 0x7FFFFFFFu);
             const int off = r_dist - (int)v[c][6], blen = (int)(v[c][7] - v[c][6]);
-            dist[c] = r_strand ? (blen - 1 - off) : off;                    // 1780-1788
-            if (dist[c] >= 2) {
-              const int np = (p[c] + dist[c] >= l - k) ? (l - k) : (p[c] + dist[c]);   // 1793-1798
-              p2[c] = rv.next_valid(np);                                    // kit2 += nextPos-pos (adv 0: p itself)
-              if (p2[c] < 0) {
+            const int dist = r_strand ? (blen - 1 - off) : off;               // 1780-1788
+            if (dist >= 2) {
+              const int np = (p[c] + dist >= l - k) ? (l - k) : (p[c] + dist);   // 1793-1798
+              const int p2 = rv.next_valid(np);                               // kit2 += nextPos-pos (adv 0: p itself)
+              if (p2 < 0) {
                 end_chain = true;                                           // 1882-1886
               } else {
                 cw(C_NP, c) = (uint32_t)np;
-                hu[c] = r_unitig; he[c] = r_ec;
+                cw(C_P2, c) = (uint32_t)p2;
+                cw(C_DIST, c) = (uint32_t)dist;
+                cw(C_HU, c) = r_unitig; cw(C_HE, c) = r_ec;
                 st[c] = S_JUMP;
                 need_prep[c] = true;
               }
@@ -699,28 +740,30 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             }
           }
         } else if (st[c] == S_JUMP) {
-          const bool found2 = !f || (hu[c] == r_unitig && he[c] == r_ec);   // 1807-1815
-          const int found2pos = !f ? p[c] : p[c] + dist[c];
+          const bool found2 = !f || (cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec);   // 1807-1815
+          const int dist = (int)cw(C_DIST, c);
+          const int found2pos = !f ? p[c] : p[c] + dist;
           if (found2) {
             if (found2pos >= l - k) end_chain = true;                       // "fake position", break (1819-1822)
-            else nv_from = p2[c] + 1;                                       // kit = kit2; ++kit
+            else nv_from = (int)cw(C_P2, c) + 1;                            // kit = kit2; ++kit
           } else {
             cw(C_H2U, c) = r_unitig; cw(C_H2E, c) = r_ec;
-            if (dist[c] > 4) {
+            if (dist > 4) {
               const int middlePos = (p[c] + (int)cw(C_NP, c)) / 2;
-              p3[c] = rv.next_valid(middlePos);                             // kit3 += middlePos-pos
-              if (p3[c] >= 0) { st[c] = S_MIDDLE; need_prep[c] = true; }
+              const int p3 = rv.next_valid(middlePos);                      // kit3 += middlePos-pos
+              if (p3 >= 0) { cw(C_P3, c) = (uint32_t)p3; st[c] = S_MIDDLE; need_prep[c] = true; }
               else to_backoff = true;
             } else {
               to_backoff = true;
             }
           }
         } else if (st[c] == S_MIDDLE) {
-          const bool foundMiddle = f && ((hu[c] == r_unitig && he[c] == r_ec) || (cw(C_H2U, c) == r_unitig && cw(C_H2E, c) == r_ec));
+          const bool foundMiddle = f && ((cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec) ||
+                                         (cw(C_H2U, c) == r_unitig && cw(C_H2E, c) == r_ec));
           if (foundMiddle) {
             push = true;
             if ((int)cw(C_NP, c) >= l - k) end_chain = true;               // 1867
-            else nv_from = p2[c] + 1;                                       // kit = kit2; ++kit
+            else nv_from = (int)cw(C_P2, c) + 1;                            // kit = kit2; ++kit
           } else {
             to_backoff = true;
           }
@@ -760,19 +803,9 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
       }
     }
   }
-  // statistics: probes and slot visits
-  n_probes += pv & 0xFFFFu;
-  n_visits += pv >> 16;
-  for (int o = 16; o > 0; o >>= 1) {
-    n_probes += __shfl_xor_sync(0xFFFFFFFFu, n_probes, o);
-    n_visits += __shfl_xor_sync(0xFFFFFFFFu, n_visits, o);
-    n_memo += __shfl_xor_sync(0xFFFFFFFFu, n_memo, o);
-  }
-  if (lane == 0 && n_probes) {
-    atomicAdd(&dd.stats[0], (unsigned long long)n_probes);
-    atomicAdd(&dd.stats[3], (unsigned long long)n_visits);
-    if (n_memo) atomicAdd(&dd.stats[2], (unsigned long long)n_memo);
-  }
+  // statistics: lookups, slot visits, memo hits (every warp leaves the loop with all its fragments finalised)
+  __syncthreads();
+  if (tid < 3 && s_tot[tid]) atomicAdd(&dd.stats[tid == 0 ? 0 : (tid == 1 ? 3 : 2)], s_tot[tid]);
 #ifdef KB_MATCH_STATS
   for (int i = 0; i < MS_N; ++i) {
     const bool per_warp = i == MS_WARP_ITERS || i == MS_SERVICE_ROUNDS || i == MS_CYCLES_LOOKUP || i == MS_CYCLES_SERVICE;

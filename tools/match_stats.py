@@ -1,7 +1,10 @@
 #!/usr/bin/env python
 """Where match_kernel's iterations go, on the benchmark workload: builds the library with -DKB_MATCH_STATS into a
 temporary directory (the in-tree build is untouched), runs the benchmark batches once and prints one JSON line with
-the summed per-launch counters and their shares.  The counters slow the kernel, so its times are not reported; the counts themselves do not depend on that."""
+the summed per-launch counters and their shares.  The counters slow the kernel, so its times are not reported; the counts themselves do not depend on that.
+The clock split of a lookup iteration (keys and hashes / the wait for the filter and slot loads / the state transitions)
+is given in cycles per lane-iteration.  KB_NVCC_DEFS adds defines to the build (e.g. -DKB_MATCH_MIN_BLOCKS=4); a
+library built beforehand with -DKB_MATCH_STATS (and those defines) can be named by KB_LIB_PATH instead."""
 import json
 import os
 import subprocess
@@ -15,13 +18,18 @@ sys.path.insert(0, ROOT)
 def build(out_dir):
     lib = os.path.join(out_dir, "libkallisto_b200.so")
     subprocess.check_call(["make", "-C", os.path.join(ROOT, "kallisto_b200", "csrc"), "-j8", lib, "OUT=" + lib,
-                           "OBJDIR=" + os.path.join(out_dir, "obj"), "NVCC=nvcc -DKB_MATCH_STATS"], stdout=subprocess.DEVNULL)
+                           "OBJDIR=" + os.path.join(out_dir, "obj"), "NVCC=nvcc -DKB_MATCH_STATS " + os.environ.get("KB_NVCC_DEFS", "")], stdout=subprocess.DEVNULL)
     return lib
 
 
 def main():
-    tmp = tempfile.mkdtemp(prefix="kb_match_stats_")
-    os.environ["KB_LIB_PATH"] = build(tmp)
+    with tempfile.TemporaryDirectory(prefix="kb_match_stats_") as tmp:
+        run(tmp)
+
+
+def run(tmp):
+    if not os.environ.get("KB_LIB_PATH"):
+        os.environ["KB_LIB_PATH"] = build(tmp)
     import torch
     import bench
     import benchdata
@@ -54,13 +62,15 @@ def main():
     lane = max(1, tot["chain_iters"])
     main_miss = tot["main_miss_filter"] + tot["main_miss_slot"]
     runs = {k: v for k, v in tot.items() if k.startswith("run_")}
-    out = {"launches": steps, "pairs": steps * P, **tot,
+    out = {"defs": os.environ.get("KB_NVCC_DEFS", ""), "launches": steps, "pairs": steps * P, **tot,
            "n_probes": st["n_probes"], "n_slot_visits": st["n_slot_visits"],
            "main_miss_lookups": main_miss,
            "share_main_miss_of_lookups": main_miss / max(1, st["n_probes"]),
            "share_main_miss_of_chain_iters": main_miss / lane,
            "live_chains_per_warp_iter": tot["chain_iters"] / max(1, tot["warp_iters"]),
            "service_share_of_cycles": tot["cycles_service"] / max(1, tot["cycles_service"] + tot["cycles_lookup"]),
+           "cycles_per_warp_iter": tot["cycles_lookup"] / max(1, tot["warp_iters"]),
+           "cycles_per_lane_iter": {p: tot["cycles_" + p] / max(1, tot["lane_iters"]) for p in ("key", "wait", "step")},
            "miss_runs": sum(runs.values())}
     print(json.dumps(out), flush=True)
     ix.close()
