@@ -305,6 +305,15 @@ int kb_bus_begin_sample(kb_quant* q, uint64_t barcode);
 /* Observed barcode / UMI length histograms (33 bins), for the header of output.bus
  * (src/main.cpp:2470-2508). */
 int kb_bus_lengths(kb_quant* q, uint32_t* bc_hist, uint32_t* umi_hist);
+/* `kallisto bus --aa` (src/ProcessReads.cpp:1652-1695, MinCollector::intersectKmersCFC src/MinCollector.cpp:44-119):
+ * on != 0 matches every read set's sequence in its six reading frames, translated into comma-free code, against an
+ * index built with `kallisto index --aa`; the frame with the smallest non-empty set wins (the lowest frame on a tie), and
+ * with a strand mode the set is then filtered by the strand of frame 0's first mapping k-mer.  Call before the first
+ * batch.  Fails for a paired technology, a tag sequence and an index with a D-list. */
+int kb_bus_set_aa(kb_quant* q, int32_t on);
+/* --aa: cardinality_clashes of the run so far ("n_frame_clashes" of run_info.json): per read set, the frames whose set
+ * is as small as the smallest one before them. */
+int kb_bus_frame_clashes(kb_quant* q, uint64_t* n_out);
 
 /* Host-only: parse a FASTA/FASTQ file (plain or gzip) with the library's reader (kseq_read grammar,
  * src/kseq.h) and report the number of records, of bases, and an FNV-1a hash of the sequences

@@ -639,6 +639,16 @@ int kb_bus_lengths(kb_quant* q, uint32_t* bc_hist, uint32_t* umi_hist) {
   return guarded([&] { q->q->bus_lengths(bc_hist, umi_hist); });
 }
 
+int kb_bus_set_aa(kb_quant* q, int32_t on) {
+  if (!q) return fail(KB_ERR_INVALID, "kb_bus_set_aa: null argument");
+  return guarded([&] { q->q->set_aa(on != 0); });
+}
+
+int kb_bus_frame_clashes(kb_quant* q, uint64_t* n_out) {
+  if (!q || !n_out) return fail(KB_ERR_INVALID, "kb_bus_frame_clashes: null argument");
+  return guarded([&] { *n_out = q->q->frame_clashes(); });
+}
+
 int kb_fastx_summary(const char* path, uint64_t* n_reads, uint64_t* n_bases, uint64_t* fnv1a) {
   return kb_fastx_summary_mt(path, 1, n_reads, n_bases, fnv1a);
 }

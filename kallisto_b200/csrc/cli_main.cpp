@@ -32,13 +32,15 @@
 #include "../../include/kallisto_b200.h"
 // Bound weakly: the command line also links against stand-ins of the library that carry only the entry points of the
 // host pipeline (tests/stub); there `quant-tcc -b`, `quant-tcc -g / -G` and --priors report the missing entry point
-// instead of failing to link.
+// instead of failing to link; so does `bus --aa`.
 #pragma weak kb_tcc_bootstrap_run
 #pragma weak kb_tcc_run_genes
 #pragma weak kb_tcc_bootstrap_run_genes
 #pragma weak kb_read_priors
 #pragma weak kb_em_set_priors
 #pragma weak kb_tcc_run_priors
+#pragma weak kb_bus_set_aa
+#pragma weak kb_bus_frame_clashes
 #include "fastx.hpp"
 #include "h5_reader.hpp"
 #include "h5_writer.hpp"
@@ -318,8 +320,10 @@ void write_abundance(const std::string& path, const std::vector<std::string>& na
 }
 
 // plaintext_aux, src/PlaintextWriter.cpp:140-199
+// frame_clashes: `bus --aa` only, the last field "n_frame_clashes" (src/PlaintextWriter.cpp:189-195)
 void write_run_info(const std::string& path, size_t n_targets, int n_bootstrap, uint64_t n_processed, uint64_t n_aln,
-                    uint64_t n_unique, int index_version, int k, const std::string& start_time, const std::string& call) {
+                    uint64_t n_unique, int index_version, int k, const std::string& start_time, const std::string& call,
+                    const std::string& frame_clashes = "") {
   std::ofstream of(path);
   double p_uniq = 0.0, p_aln = 0.0;
   if (n_processed > 0) {
@@ -343,9 +347,12 @@ void write_run_info(const std::string& path, size_t n_targets, int n_bootstrap, 
      << to_json("kallisto_version", KALLISTO_VERSION, true) << std::endl
      << to_json("index_version", std::to_string(index_version), false) << std::endl
      << to_json("k-mer length", std::to_string(k), false) << std::endl
-     << to_json("start_time", start_time, true) << std::endl
-     << to_json("call", call, true, false) << std::endl
-     << "}" << std::endl;
+     << to_json("start_time", start_time, true) << std::endl;
+  if (!frame_clashes.empty())
+    of << to_json("call", call, true) << std::endl << to_json("n_frame_clashes", frame_clashes, false, false) << std::endl;
+  else
+    of << to_json("call", call, true, false) << std::endl;
+  of << "}" << std::endl;
 }
 
 #define KB_TRY(x)                                                     \
@@ -1051,6 +1058,8 @@ void usage_bus() {
             << "    --batch=FILE              Process files listed in FILE (lines: id file1 [file2]), one sample per" << endl
             << "                              line; without a technology only" << endl
             << "    --fr-stranded / --rf-stranded / --unstranded   Strand specificity" << endl
+            << "    --aa                      Align to index generated from a FASTA-file containing amino acid sequences" << endl
+            << "                              (single-end reads; not with --tag or an index with a D-list)" << endl
             << "    --device=INT              CUDA device ordinal (default: 0)" << endl;
 }
 
@@ -1058,10 +1067,14 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   Options opt;
   std::string technology, tagsequence, batch_file;
   int num_flag = 0, fr = 0, rf = 0, unstranded = 0, verbose_flag = 0, paired_flag = 0, interleaved_flag = 0;
+  int aa_flag = 0, union_flag = 0, no_jump_flag = 0;
   const char* opt_string = "i:o:x:t:nD:T:B:";
   static struct option long_options[] = {{"verbose", no_argument, &verbose_flag, 1},
                                          {"paired", no_argument, &paired_flag, 1},
                                          {"inleaved", no_argument, &interleaved_flag, 1},
+                                         {"aa", no_argument, &aa_flag, 1},
+                                         {"union", no_argument, &union_flag, 1},
+                                         {"no-jump", no_argument, &no_jump_flag, 1},
                                          {"tag", required_argument, 0, 'T'},
                                          {"batch", required_argument, 0, 'B'},
                                          {"num", no_argument, 0, 'n'},
@@ -1268,6 +1281,18 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
       bo.tag = tagsequence.c_str();
     }
   }
+  // --union / --no-jump are not built here; with --aa the reference refuses them as well (src/main.cpp:969-976)
+  if (union_flag) { cerr << (aa_flag ? "--union is not compatible with this mode" : "Error: --union is not supported by this build") << endl; ret = false; }
+  if (no_jump_flag) { cerr << (aa_flag ? "--no-jump is not compatible with this mode" : "Error: --no-jump is not supported by this build") << endl; ret = false; }
+  if (aa_flag) {
+    // the reference turns --paired off with a note and matches the first sequence read alone (src/main.cpp:761-770);
+    // this build says so instead of dropping a read
+    if (paired_flag || bo.paired) {
+      cerr << "Error: --aa supports single-end reads only: --paired and technologies with two sequence reads are not supported" << endl;
+      ret = false;
+    }
+    if (!tagsequence.empty()) { cerr << "Error: --aa with a UMI tag sequence (--tag) is not supported" << endl; ret = false; }
+  }
   if (opt.output.empty()) { cerr << "Error: need to specify output directory " << opt.output << endl; ret = false; }
   else if (stat(opt.output.c_str(), &stt) == 0) {
     if (!S_ISDIR(stt.st_mode)) { cerr << "Error: file " << opt.output << " exists and is not a directory" << endl; ret = false; }
@@ -1296,6 +1321,10 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   bo.max_batch_bases = 2 * max_bases;
   kb_quant* q = nullptr;
   KB_TRY(kb_bus_create(ix, &bo, &q));
+  if (aa_flag) {
+    if (!kb_bus_set_aa || !kb_bus_frame_clashes) { cerr << "Error: this libkallisto_b200 has no kb_bus_set_aa" << endl; return 1; }
+    KB_TRY(kb_bus_set_aa(q, 1));      // refuses an index with a D-list
+  }
   auto spec_len = [](const kb_bus_substr* v, int n) {   // BUSOptions::getBCLength / getUMILength
     int r = 0;
     for (int i = 0; i < n; ++i) {
@@ -1427,8 +1456,14 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
     std::ofstream tf(opt.output + "/transcripts.txt");
     for (uint32_t i = 0; i < info.n_targets; ++i) tf << kb_index_target_name(ix, i) << "\n";
   }
+  std::string frame_clashes;
+  if (aa_flag) {
+    uint64_t nc = 0;
+    KB_TRY(kb_bus_frame_clashes(q, &nc));
+    frame_clashes = std::to_string(nc);
+  }
   write_run_info(opt.output + "/run_info.json", info.n_targets, 0, st.n_processed, st.n_pseudoaligned, st.n_unique, 13, info.k,
-                 start_time, call);
+                 start_time, call, frame_clashes);
   cerr << endl;
   if (!getenv("KB_CLI_CLEANUP")) finish(st.n_pseudoaligned == 0 ? 1 : 0);
   free_streams(streams);

@@ -517,7 +517,7 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ba.fixed_len = fixed_len;
   ba.n_frag = n_frag;
   ba.paired = opt_.paired;
-  ba.strand_mode = opt_.strand_mode;
+  ba.strand_mode = aa_ ? 0 : opt_.strand_mode;     // --aa: the frames are matched unstranded, cfc_select_kernel filters the set
   ba.frag_base = have_frag_base_ ? frag_base_ : n_frag_total_;
   have_frag_base_ = false;
   ba.handle_out = bws_->d_handles.p;
@@ -558,6 +558,8 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ba.notag = cur_notag_;
   ba.alt_start = cur_alt_start_;
   ba.alt_start2 = cur_alt_start2_;
+  ba.no_count = aa_ ? 1 : 0;
+  ba.first_hit = aa_ ? cfc_first_.p : nullptr;
   ResolveArgs ra{};
   ra.scratch = bws_->d_scratch.p;
   ra.scratch_stride = scratch_stride_;
@@ -578,6 +580,11 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   launch_pseudoalign(ix_.dev, dd_, ba, ra, tpb, stream_, ev);
   KB_CK(cudaGetLastError());
   n_kernel_launches += 3 + (ba.skip_w ? 1 : 0);   // pack_kernel, [dlist_scan_kernel,] match_kernel, resolve_kernel
+  if (aa_) {
+    launch_cfc_select(ix_.dev, dd_, ba, ra, n_frag / 6, opt_.strand_mode, cfc_handles_.p, cfc_clashes_.p, stream_);
+    KB_CK(cudaGetLastError());
+    ++n_kernel_launches;
+  }
   if (want_fld) {
     launch_fld_finalize(dd_, ba, stream_);
     ++n_kernel_launches;
@@ -593,7 +600,7 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
     }
     tlencount_ += local;
   }
-  n_frag_total_ += n_frag;
+  n_frag_total_ += aa_ ? n_frag / 6 : n_frag;     // --aa: read sets are counted, not their frames
 }
 
 void Quant::pseudoalign_device(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
@@ -773,9 +780,41 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   }
   maxlen = maxlen > min_start ? maxlen - min_start : 1;
   const uint64_t base = n_frag_total_;
+  const int32_t* handles = bws_->d_handles.p;
   cur_skip_ = bus_skip_.p;
   cur_start_ = (uint32_t)sp.seq_start;
-  if (sp.paired) {
+  if (aa_) {
+    // the six reading frames of every set in comma-free code (kernels_cfc.cu), 6 n_sets unpaired fragments; a skipped
+    // set has empty frames
+    const uint64_t bound = 6ull * n_sets * maxlen;
+    if (bound >= (1ull << 32)) throw Error("kallisto_b200: bus --aa batch too large (6 x read sets x longest read must be < 2^32)");
+    auto grow_to = [&](auto& b, size_t need, size_t dflt) { if (b.n < need) b.alloc(std::max(need, dflt)); };
+    grow_to(cfc_b_, bound + 16, 0);
+    grow_to(cfc_o_, 6 * (size_t)n_sets + 1, 6 * (size_t)opt_.max_batch_reads + 1);
+    grow_to(cfc_first_, 6 * (size_t)n_sets, 6 * (size_t)opt_.max_batch_reads);
+    grow_to(cfc_set_off_, n1, (size_t)opt_.max_batch_reads + 1);
+    grow_to(cfc_handles_, n1, (size_t)opt_.max_batch_reads + 1);
+    grow_to(cfc_tmp_, cfc_scan_bytes(n_sets), cfc_scan_bytes(opt_.max_batch_reads));
+    CfcArgs c{};
+    c.bases = db[sp.seq_file];
+    c.off = dofs[sp.seq_file];
+    c.start = (uint32_t)sp.seq_start;
+    c.skip = bus_skip_.p;
+    c.n_sets = n_sets;
+    c.max_len = maxlen;
+    c.set_off = cfc_set_off_.p;
+    c.fbases = cfc_b_.p;
+    c.foff = cfc_o_.p;
+    c.tmp = cfc_tmp_.p;
+    c.tmp_bytes = cfc_tmp_.n;
+    launch_cfc_frames(c, st);
+    KB_CK(cudaGetLastError());
+    n_kernel_launches += 2;      // cfc_len, cfc_frames
+    cur_skip_ = nullptr;
+    cur_start_ = 0;
+    run_batch(cfc_b_.p, cfc_o_.p, 6 * n_sets, 0, maxlen);
+    handles = cfc_handles_.p;
+  } else if (sp.paired) {
     // two sequence reads (busopt.paired, src/ProcessReads.cpp:1550-1567,1646-1650): the pair goes through the same
     // match x 2 / intersectKmers / strand filter / mapPair path as `quant` (one buffer per mate)
     cur_start2_ = (uint32_t)sp.seq2_start;
@@ -788,7 +827,7 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   cur_start2_ = 0;
   cur_notag_ = nullptr;
   cur_alt_start_ = cur_alt_start2_ = 0;
-  launch_bus_records(dd_, bws_->d_handles.p, n_sets, base, bus_next_id_, bus_idof_.p, bus_isnew_.p, bus_newrank_.p,
+  launch_bus_records(dd_, handles, n_sets, base, bus_next_id_, bus_idof_.p, bus_isnew_.p, bus_newrank_.p,
                      bus_ismapped_.p, bus_rank_.p, (const uint64_t*)bus_bc_.p, (const uint64_t*)bus_umi_.p, bus_flags_.p,
                      bus_rec_.p, bus_tmp_.p, bus_tmp_.n, st);
   KB_CK(cudaGetLastError());
@@ -813,6 +852,36 @@ void Quant::bus_begin_sample(uint64_t barcode) {
   std::fill(flens_.begin(), flens_.end(), 0u);
   tl_list_.clear();
   tlencount_ = 0;
+}
+
+void Quant::set_aa(bool on) {
+  KB_CK(cudaSetDevice(ix_.device));
+  if (!opt_.bus) throw Error("kallisto_b200: --aa needs a bus run");
+  if (n_frag_total_ != 0) throw Error("kallisto_b200: --aa must be chosen before the first batch");
+  if (on) {
+    if (opt_.paired || opt_.bus_spec.paired)
+      throw Error("kallisto_b200: --aa translates single-end reads only; a paired technology or --paired is not supported");
+    if (opt_.bus_spec.tag_len) throw Error("kallisto_b200: --aa with a UMI tag sequence (--tag) is not supported");
+    if (ix_.dev.dfk)
+      throw Error("kallisto_b200: --aa with an index that has a D-list is not supported: there the reference keeps the off-list "
+                  "target in every frame's intersection (dfk_onlist), which makes the result depend on the order of the hits");
+    // 6 frames per read set go through the pseudoalignment buffers
+    const size_t frames = 6 * (size_t)opt_.max_batch_reads;
+    bws_->d_handles.grow(frames);
+    bws_->d_qentries.grow(frames * KB_Q_STRIDE);
+    cfc_clashes_.grow(1);
+    cfc_clashes_.zero(stream_);
+  }
+  aa_ = on;
+}
+
+uint64_t Quant::frame_clashes() {
+  unsigned long long c = 0;
+  if (aa_) {
+    cfc_clashes_.download(&c, 1, 0, stream_);
+    KB_CK(cudaStreamSynchronize(stream_));
+  }
+  return c;
 }
 
 void Quant::bus_lengths(uint32_t* bc_hist, uint32_t* umi_hist) {

@@ -228,6 +228,12 @@ class Quant {
   // Batch mode (`bus -x BULK`, src/ProcessReads.cpp:371-404,1603-1607): the read sets that follow belong to sample
   // `barcode` (the fake barcode of their records); its fragment-length sampling starts from an empty histogram.
   void bus_begin_sample(uint64_t barcode);
+  // `bus --aa` (src/ProcessReads.cpp:1652-1695): every read set is matched in its six reading frames, translated into
+  // comma-free code, against a protein index; the smallest non-empty frame set wins.  Before the first batch; refused
+  // for paired technologies, tag sequences and indices with a D-list.
+  void set_aa(bool on);
+  // cardinality_clashes of the run: frames whose set was as small as the winning frame's before them
+  uint64_t frame_clashes();
   // Same, inputs already resident in device memory; handles stay on the device
   // (device_handles(), valid until the next batch).
   void pseudoalign_device(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
@@ -360,6 +366,12 @@ class Quant {
   const uint8_t* cur_skip_ = nullptr;
   uint32_t cur_start_ = 0, cur_start2_ = 0, cur_alt_start_ = 0, cur_alt_start2_ = 0;
   const uint8_t* cur_notag_ = nullptr;
+  // bus --aa: the frames of a batch (6 per read set), frame 0's first hit per set, the sets' handles, the clash count
+  bool aa_ = false;
+  DBuf<uint8_t> cfc_b_, cfc_tmp_;
+  DBuf<uint32_t> cfc_o_, cfc_set_off_, cfc_first_;
+  DBuf<int32_t> cfc_handles_;
+  DBuf<unsigned long long> cfc_clashes_;
 };
 
 std::vector<double> mean_fl_trunc_of(const uint32_t* flens /* 1000 */, double fld_mean, double fld_sd);

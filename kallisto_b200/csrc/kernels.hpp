@@ -69,6 +69,12 @@ struct BatchArgs {
   // fragments sample fragment lengths.  nullptr = no tag sequence in play.
   const uint8_t* notag;
   uint32_t alt_start, alt_start2;
+  // Translated search (bus --aa): the fragments are the six reading frames of each read set, and cfc_select_kernel
+  // accounts for the set.  no_count != 0: match_kernel and resolve_kernel leave dd.count and dd.first alone.
+  // first_hit (optional): per fragment, block * 2 + orientation of the first k-mer found (the first mapping k-mer of
+  // doStrandSpecificity), or 0xFFFFFFFF when there is none.
+  int no_count;
+  uint32_t* first_hit;
 };
 static constexpr int KB_Q_STRIDE = 2 + KB_MAX_E + 6;   // frag, n|flags, handles, 2 strand words, 4 position-filter words
 static constexpr int KB_SPILL = 112;                   // a fragment may hit KB_MAX_E + KB_SPILL = 128 distinct EC sets
@@ -338,6 +344,30 @@ void launch_bus_records(const DevDict& dd, const int32_t* handle, uint32_t n, ui
                         int32_t* id_of, uint32_t* is_new, uint32_t* new_rank, uint32_t* is_mapped, uint32_t* rank,
                         const uint64_t* barcode, const uint64_t* umi, const uint32_t* flags, BusRecord* out, void* tmp,
                         size_t tmp_bytes, cudaStream_t st);
+
+// ---- translated search, bus --aa (kernels_cfc.cu) ----
+// The six reading frames of every read set in comma-free code, fragment 6 i + j = frame j of set i.
+struct CfcArgs {
+  const uint8_t* bases;     // the sequence file of the batch
+  const uint32_t* off;      // n_sets + 1
+  uint32_t start;           // first base of the sequence in its read
+  const uint8_t* skip;      // per set: 1 = no sequence (bad barcode / UMI): its frames are empty
+  uint32_t n_sets;
+  uint32_t max_len;         // longest sequence (after `start`)
+  uint32_t* set_off;        // n_sets + 1: frame letters before each set (filled by launch_cfc_frames)
+  uint8_t* fbases;          // frame letters
+  uint32_t* foff;           // 6 n_sets + 1 frame offsets
+  void* tmp;
+  size_t tmp_bytes;         // cfc_scan_bytes(n_sets)
+};
+size_t cfc_scan_bytes(uint32_t n_sets);
+void launch_cfc_frames(const CfcArgs& a, cudaStream_t st);
+// After the frames went through launch_pseudoalign with ba.no_count and ba.first_hit: per set, the winning frame's set
+// (smallest non-empty, lowest frame on a tie), the frame-0 strand filter when strand_mode != 0, the accounting
+// (dd.count, dd.first = ba.frag_base + set) and the set's handle in handle_out[set].  clashes += frames whose set is as
+// small as the smallest one before them.
+void launch_cfc_select(const DevIndex& ix, const DevDict& dd, const BatchArgs& ba, const ResolveArgs& ra, uint32_t n_sets,
+                       int strand_mode, int32_t* handle_out, unsigned long long* clashes, cudaStream_t st);
 
 struct ResampleArgs {
   const double* cp;          // n_ec cumulative probabilities (discrete_distribution::_M_cp)

@@ -18,6 +18,7 @@
 // src/MinCollector.cpp:251-269): EC ids are assigned afterwards in order of first occurrence,
 // which is what the reference produces with -t 1.
 #include "kb_device.cuh"
+#include "kb_dict.cuh"
 #include "kernels.hpp"
 
 #ifndef KB_MATCH_MIN_BLOCKS
@@ -61,11 +62,6 @@ __device__ __forceinline__ int run_bin(int n) {
 
 namespace {
 
-__device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ int32_t ld_relaxed_s32(const int32_t* p) {
   int32_t v;
   asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -552,9 +548,10 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
           ba.tl_out[frag] = tl;
         }
         // per-handle accounting, aggregated over the lanes finalised in this round
+        if (ba.first_hit) ba.first_hit[frag] = v0 ? f_blk[0] * 2u + (f_ds[0] >> 31) : 0xFFFFFFFFu;
         const unsigned grp = __match_any_sync(fin, handle);
         const uint32_t fmin = __reduce_min_sync(grp, frag);
-        if (handle >= 0 && lane == (unsigned)(__ffs(grp) - 1)) {
+        if (handle >= 0 && !ba.no_count && lane == (unsigned)(__ffs(grp) - 1)) {
           atomicAdd(&dd.count[handle], (uint32_t)__popc(grp));
           atomicMin(&dd.first[handle], (unsigned long long)(ba.frag_base + fmin));
         }
@@ -817,81 +814,6 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
 #endif
 }
 
-namespace {
-
-__device__ __forceinline__ bool bsearch_contains(const uint32_t* s, uint32_t n, uint32_t v, uint32_t* rank) {
-  uint32_t lo = 0, hi = n;
-  while (lo < hi) {
-    const uint32_t mid = (lo + hi) >> 1;
-    const uint32_t x = __ldcg(s + mid);
-    if (x < v) lo = mid + 1; else hi = mid;
-  }
-  if (rank) *rank = lo;
-  return lo < n && __ldcg(s + lo) == v;
-}
-
-// Lane groups: G consecutive lanes of a warp (G = 32, 16, 8 or 4) work on one item; the groups of a warp are
-// independent of each other (every collective below names only the group's lanes).
-template <int G>
-__device__ __forceinline__ unsigned group_mask(unsigned lane_in_warp) {
-  return G == 32 ? 0xFFFFFFFFu : (((1u << (G & 31)) - 1u) << (lane_in_warp & ~(unsigned)(G - 1)));
-}
-
-// Group-cooperative lookup-or-insert of a sorted transcript-id list in the content-addressed set
-// dictionary (ecmapinv semantics: equal sets share one handle).  `src` may be shared or global memory
-// readable by all lanes of the group; `lane` is the lane's index inside its group, `gmask` the group's lanes.
-// Returns the handle, or KB_H_UNMAPPED after flagging an error.
-template <int G = 32>
-__device__ __forceinline__ int32_t dict_insert_warp(const DevDict& dd, const uint32_t* src, uint32_t nres, unsigned lane,
-                                                    unsigned gmask = 0xFFFFFFFFu) {
-  uint64_t sum = 0;
-  for (uint32_t i = lane; i < nres; i += G) sum += kb_mix64((uint64_t)src[i] + 0x9E3779B97F4A7C15ULL);
-  for (int o = G / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(gmask, sum, o);
-  const uint64_t hsh = kb_mix64(sum ^ nres);
-  const unsigned long long tag = hsh >> 56;
-  uint64_t s = hsh & dd.dmask;
-  unsigned long long my_word = ~0ULL;   // pool space is allocated lazily
-  uint64_t visited = 0;
-  for (;;) {
-    unsigned long long word = 0;
-    if (lane == 0) word = ld_acquire_u64(&dd.dslots[s]);
-    word = __shfl_sync(gmask, word, 0, G);
-    if (word == ~0ULL) {
-      if (my_word == ~0ULL) {
-        unsigned long long off = 0;
-        if (lane == 0) off = atomicAdd(dd.pool_top, (unsigned long long)nres);
-        off = __shfl_sync(gmask, off, 0, G);
-        if (off + nres > dd.pool_cap || off + nres > 0xFFFFFFFFULL) {
-          if (lane == 0) atomicOr(dd.error, KB_DEVERR_POOL_FULL);
-          return KB_H_UNMAPPED;
-        }
-        for (uint32_t i = lane; i < nres; i += G) dd.pool[off + i] = src[i];
-        __threadfence();
-        __syncwarp(gmask);
-        my_word = off | ((unsigned long long)nres << 32) | (tag << 56);
-      }
-      unsigned long long old = 0;
-      if (lane == 0) old = atomicCAS(&dd.dslots[s], ~0ULL, my_word);
-      old = __shfl_sync(gmask, old, 0, G);
-      if (old == ~0ULL) return (int32_t)s;
-      word = old;   // somebody else took the slot: compare against theirs
-    }
-    if ((word >> 56) == tag && ((word >> 32) & 0xFFFFFFu) == nres) {
-      const uint32_t* S = dd.pool + (uint32_t)word;
-      bool eq = true;
-      for (uint32_t i = lane; i < nres; i += G) eq = eq && (__ldcg(S + i) == src[i]);
-      if (__all_sync(gmask, eq)) return (int32_t)s;
-    }
-    s = (s + 1) & dd.dmask;
-    if (++visited > dd.dmask) {
-      if (lane == 0) atomicOr(dd.error, KB_DEVERR_DICT_FULL);
-      return KB_H_UNMAPPED;
-    }
-  }
-}
-
-}  // namespace
-
 // One group of G lanes per queued fragment (ra.n_warps counts groups).  The kernel is a chain of dependent memory
 // accesses per fragment (queue entry -> memo -> set descriptors -> set elements -> binary searches -> dictionary ->
 // memo), so what sets its speed is the number of fragments in flight: the sets are short (2.5 ids on average), 8
@@ -1097,7 +1019,7 @@ __global__ void __launch_bounds__(128, 8) resolve_kernel(DevIndex ix, DevDict dd
     // 6. account for this fragment
     if (lane == 0) {
       ba.handle_out[f] = handle;
-      if (handle >= 0) {
+      if (handle >= 0 && !ba.no_count) {
         atomicAdd(&dd.count[handle], 1u);
         atomicMin(&dd.first[handle], (unsigned long long)(ba.frag_base + f));
       }
