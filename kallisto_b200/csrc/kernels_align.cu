@@ -42,13 +42,16 @@ enum : int {
   // split of a lane-iteration's cycles, summed over lanes (cycles_lookup and cycles_service are lane 0's): keys and hashes
   // up to the filter loads, the wait for the filter and slot loads, and the state transitions (with the handle dedup)
   MS_CYCLES_KEY, MS_CYCLES_WAIT, MS_CYCLES_STEP,
+  // chain iterations settled on the straight-line path (collision, MAIN miss on a mate without N), and the passes of the
+  // general transition per warp-iteration (summed over warps; a warp runs as many as its busiest lane needs)
+  MS_STRAIGHT, MS_GEN_PASSES,
   MS_RUN_HIST, MS_N = MS_RUN_HIST + 9     // MAIN miss runs of 1, 2, 3, 4, 5-8, 9-16, 17-32, 33-64, 65+ positions
 };
 __device__ unsigned long long kb_match_stats[MS_N];
 static const char* const kMatchStatNames[MS_N] = {
   "warp_iters", "service_rounds", "lane_iters", "chain_iters",
   "main_hit", "main_miss_filter", "main_miss_slot", "jump", "middle", "backoff", "collision",
-  "cycles_lookup", "cycles_service", "cycles_key", "cycles_wait", "cycles_step",
+  "cycles_lookup", "cycles_service", "cycles_key", "cycles_wait", "cycles_step", "straight", "gen_passes",
   "run_1", "run_2", "run_3", "run_4", "run_5_8", "run_9_16", "run_17_32", "run_33_64", "run_65_"};
 __device__ __forceinline__ int run_bin(int n) {
   return n <= 4 ? n - 1 : (n <= 8 ? 4 : (n <= 16 ? 5 : (n <= 32 ? 6 : (n <= 64 ? 7 : 8))));
@@ -182,6 +185,12 @@ enum : int {
   S_MAIN = 0, S_JUMP = 1, S_MIDDLE = 2, S_BACKOFF = 3,   // k-mer table lookups (KmerIndex::match control flow)
   S_FIN = 4,                                             // chain ended; the fragment waits for the next service round once both have
   S_EMPTY = 5                                            // no fragment assigned
+};
+// What a chain's next lookup does to its k-mer before the probe.
+enum : int {
+  P_NONE = 0,      // nothing: the same key at the next slot (linear probing)
+  P_BUILD = 1,     // read it from the packed bases at the state's position
+  P_ROLL = 2       // shift in one base: the lookup is at p + 1 of the k-mer the chain holds
 };
 // Cold words of a chain in shared memory: word w of chain c of a lane is its per-lane word KB_MAX_E + 2 * w + c.  The
 // first three (the chain's first hit) are overwritten when a finalised tuple grows past KB_MAX_E.  The rest are only
@@ -317,9 +326,12 @@ __global__ void __launch_bounds__(256) dlist_scan_kernel(DevIndex ix, BatchArgs 
 // maximum over its lanes, and lanes sitting at different call sites serialise.  Here each lane
 // keeps an explicit state per chain -- chain m matches mate m of the lane's fragment; single-end
 // reads use chain 0 only -- and every iteration of the warp's loop performs ONE lookup per live
-// chain through a single convergent site: the canonical k-mers + hashes of both chains, both
-// presence-filter loads, then both 32-byte slot loads (two 128-bit loads of the same sector on
-// sm_90a), and only then the reference's control flow as a state transition, chain 0 first
+// chain through a single convergent site: the canonical k-mers + hashes of both chains (a k-mer one
+// position after the chain's previous one is rolled from it by one base), both presence-filter
+// loads, then both 32-byte slot loads (two 128-bit loads of the same sector on sm_90a), and only
+// then the reference's control flow as a state transition.  Collisions and MAIN misses on mates
+// without N are settled for both chains by straight-line code; the other outcomes go through one
+// copy of the transition, a pass per chain that needs it, chain 0 first
 //   MAIN     the k-mer at p.  Miss: next valid k-mer.  Hit: record it, distance to the end of its EC
 //            block (1780-1788); if >= 2 go to JUMP.
 //   JUMP     the jump target (1793-1827).  Absent or same (unitig, EC set): accepted, scanning resumes
@@ -376,14 +388,17 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
   int n_e = 0;
   bool overflow = false;
   unsigned inv_flags = 0;    // bit m: mate m holds a base other than A/C/G/T
-  // per chain (index = mate); the state of a jump or middle probe and the first hit live in `cold`
+  // per chain (index = mate); the state of a jump or middle probe and the first hit live in `cold`.  The arrays are
+  // only indexed by compile-time constants (unrolled loops); code that picks a chain at run time does so by selects.
   int st[2] = {S_EMPTY, S_EMPTY};
   int p[2] = {-1, -1}, len[2] = {0, 0};
-  bool need_prep[2] = {false, false}, is_canon[2] = {false, false};
-  bool hv[2] = {false, false}, hs[2] = {false, false};   // the mate has a hit / a hit on a non-empty EC set
-  uint64_t canon[2] = {0, 0};
+  int prep[2] = {P_NONE, P_NONE};
+  unsigned hv = 0, hs = 0;     // bit m: mate m has a hit / a hit on a non-empty EC set
+  // the k-mer of the chain's current lookup and its reverse complement (the key is the smaller of the two)
+  uint64_t fwd[2] = {0, 0}, rc[2] = {0, 0};
   uint32_t slot[2] = {0, 0};   // the table has at most 2^32 slots (KmerIndex load)
   const uint32_t slot_mask = (uint32_t)ix.mask;
+  const uint64_t kmask = (1ULL << (2 * k)) - 1;
   uint32_t pv = 0;          // counter of the current fragment: lookups in the low half, slot visits in the high half
 #ifdef KB_MATCH_STATS
   unsigned long long ms[MS_N] = {};
@@ -392,14 +407,15 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
   long long t_step = -1;    // >= 0: the lane's state transitions of this lookup iteration started at this clock
   auto end_run = [&](int c) { if (run[c] > 0) { KB_MS(MS_RUN_HIST + run_bin(run[c]), 1); run[c] = 0; } };
 #endif
-  // view of mate c of the lane's fragment
-  auto view = [&](int c) {
+  // view of mate c of the lane's fragment, of length l (the caller reads len[c]: a run-time index into the array would
+  // put it in local memory)
+  auto view = [&](int c, int l) {
     ReadView rv;
     rv.bw = s_bw + (size_t)c * nw * nt;
     rv.gmask = ba.packed + (size_t)(ba.paired ? 2 * frag + c : frag) * ba.pstride + nw;
     rv.n_mask = nb;
     rv.stride = nt;
-    rv.len = len[c];
+    rv.len = l;
     rv.k = k;
     rv.has_invalid = ((inv_flags >> c) & 1u) != 0;
     return rv;
@@ -429,7 +445,7 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
       if (done) {
         bool memo_hit = false;
         // ---- MinCollector::intersectKmers, net effect (MinCollector.cpp:160-218) ----
-        const bool v0 = hv[0], s0 = hs[0], v1 = hv[1], s1 = hs[1];
+        const bool v0 = hv & 1u, s0 = hs & 1u, v1 = hv & 2u, s1 = hs & 2u;
         // first hit of each mate, before the tuple may grow over it
         uint32_t f_blk[2], f_ds[2], f_pos[2];
 #pragma unroll
@@ -613,13 +629,13 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
           n_e = 0;
           overflow = false;
           inv_flags = inv;
+          hv = hs = 0;
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
-            hv[c] = hs[c] = false;
-            need_prep[c] = true;
+            prep[c] = P_BUILD;
             st[c] = S_FIN;     // no second mate, or a mate without a valid k-mer: the chain ends here
             if (c < n_mates) {
-              p[c] = view(c).next_valid(0);
+              p[c] = view(c, len[c]).next_valid(0);
               if (p[c] >= 0) st[c] = S_MAIN;
             }
           }
@@ -632,22 +648,30 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     // ------------------------------------------------------------------ one lookup per live chain
     const bool live[2] = {st[0] <= S_BACKOFF, st[1] <= S_BACKOFF};
     KB_MS(MS_WARP_ITERS, 1);
+    KB_MS_ONLY(int n_pass = 0;)
     if (live[0] || live[1]) {
       KB_MS(MS_LANE_ITERS, 1);
       // keys of both chains and their presence-filter words (L2 resident) before either is used
       uint32_t fword[2] = {0xFFFFFFFFu, 0xFFFFFFFFu}, fbit[2] = {0, 0};
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        if (live[c] && need_prep[c]) {
+        if (live[c] && prep[c] != P_NONE) {
           const bool filtered = st[c] == S_MAIN || st[c] == S_BACKOFF;
-          const int pq = filtered ? p[c] : (int)cw(st[c] == S_JUMP ? C_P2 : C_P3, c);
-          const uint64_t fwd = view(c).kmer(pq);
-          const uint64_t rc = kb_revcomp(fwd, k);
-          is_canon[c] = fwd < rc;
-          canon[c] = is_canon[c] ? fwd : rc;
-          const uint64_t hsh = kb_mix64(canon[c]);
+          if (prep[c] == P_ROLL) {
+            // the k-mer at p from the one at p - 1: its last base enters at the low end of the forward k-mer and,
+            // complemented, at the high end of the reverse complement
+            const int q = p[c] + k - 1;
+            const uint64_t b = (s_bw[((size_t)c * nw + (q >> 4)) * nt] >> (30 - 2 * (q & 15))) & 3u;
+            fwd[c] = ((fwd[c] << 2) | b) & kmask;
+            rc[c] = (rc[c] >> 2) | ((b ^ 3u) << (2 * k - 2));
+          } else {
+            const int pq = filtered ? p[c] : (int)cw(st[c] == S_JUMP ? C_P2 : C_P3, c);
+            fwd[c] = view(c, len[c]).kmer(pq);
+            rc[c] = kb_revcomp(fwd[c], k);
+          }
+          const uint64_t hsh = kb_mix64(fwd[c] < rc[c] ? fwd[c] : rc[c]);
           slot[c] = (uint32_t)hsh & slot_mask;
-          need_prep[c] = false;
+          prep[c] = P_NONE;
           ++pv;
           // a clear bit means the k-mer is not in the index -- no HBM sector is touched.  The jump target and the
           // middle k-mer lie in the EC block of the hit before them and are nearly always present: their slot is
@@ -685,42 +709,74 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
         t_step = t_wait;
       }
 #endif
+      // the common outcomes first, for both chains and without branches: a collision moves to the next slot (linear
+      // probing), and a MAIN miss on a mate without bases other than A/C/G/T moves to the next position, whose k-mer is
+      // then rolled from this one.  Only a hit, a JUMP, MIDDLE or BACKOFF lookup, or a miss on a mate with such a base
+      // is left to the general transition below.
+      bool f[2];
+      unsigned todo = 0;     // bit c: chain c takes the general transition
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        if (!live[c]) continue;
-        KB_MS(MS_CHAIN_ITERS, 1);
         const uint64_t key = (uint64_t)v[c][0] | ((uint64_t)v[c][1] << 32);
-        if (key != canon[c] && key != KB_EMPTY_KEY) {
-          slot[c] = (slot[c] + 1) & slot_mask;      // linear probing: one more iteration
-          KB_MS(MS_COLLISION, 1);
-          continue;
-        }
-        const bool f = key == canon[c];
+        f[c] = key == (fwd[c] < rc[c] ? fwd[c] : rc[c]);
+        const bool coll = live[c] && !f[c] && key != KB_EMPTY_KEY;
+        const bool step = live[c] && !f[c] && !coll && st[c] == S_MAIN && !((inv_flags >> c) & 1u);
 #ifdef KB_MATCH_STATS
-        if (st[c] == S_MAIN) {
-          if (f) { KB_MS(MS_MAIN_HIT, 1); end_run(c); }
-          else { KB_MS(((fword[c] >> fbit[c]) & 1u) ? MS_MAIN_MISS_SLOT : MS_MAIN_MISS_FILTER, 1); ++run[c]; }
-        } else {
-          KB_MS(st[c] == S_JUMP ? MS_JUMP : (st[c] == S_MIDDLE ? MS_MIDDLE : MS_BACKOFF), 1);
+        if (live[c]) {
+          KB_MS(MS_CHAIN_ITERS, 1);
+          if (coll || step) KB_MS(MS_STRAIGHT, 1);
+          if (coll) {
+            KB_MS(MS_COLLISION, 1);
+          } else if (st[c] == S_MAIN) {
+            if (f[c]) { KB_MS(MS_MAIN_HIT, 1); end_run(c); }
+            else { KB_MS(((fword[c] >> fbit[c]) & 1u) ? MS_MAIN_MISS_SLOT : MS_MAIN_MISS_FILTER, 1); ++run[c]; }
+          } else {
+            KB_MS(st[c] == S_JUMP ? MS_JUMP : (st[c] == S_MIDDLE ? MS_MIDDLE : MS_BACKOFF), 1);
+          }
         }
 #endif
-        // hit fields: v[2] unitig, v[3] blk, v[4] ec (set handle), v[5] dist|flag, v[6] lb, v[7] ub
-        const uint32_t r_unitig = v[c][2], r_ec = v[c][4];
-        const bool r_strand = (is_canon[c] == ((v[c][5] >> 31) != 0));
-        const int l = len[c];
-        const ReadView rv = view(c);
+        if (coll) slot[c] = (slot[c] + 1) & slot_mask;
+        if (step) {
+          ++p[c];
+          prep[c] = P_ROLL;
+          if (p[c] > len[c] - k) st[c] = S_FIN;
+          KB_MS_ONLY(if (st[c] == S_FIN) end_run(c);)
+        }
+        if (live[c] && !coll && !step) todo |= 1u << c;
+      }
+      // the general transition (KmerIndex::match's control flow), one copy for both chains: each pass takes the lane's
+      // lowest chain that still needs it, its fields picked by selects.  A warp runs as many passes as its busiest lane
+      // needs, and chain 1's handle dedup sees what chain 0 pushed in the same iteration.
+      while (todo) {
+        KB_MS_ONLY(++n_pass;)
+        const bool c1 = !(todo & 1u);
+        const int c = c1 ? 1 : 0;
+        todo &= todo - 1;
+        const int s = c1 ? st[1] : st[0];
+        const int pc = c1 ? p[1] : p[0];
+        const int l = c1 ? len[1] : len[0];
+        const bool fc = c1 ? f[1] : f[0];
+        const bool is_canon = c1 ? fwd[1] < rc[1] : fwd[0] < rc[0];
+        // hit fields: h[0] unitig, h[1] blk, h[2] ec (set handle), h[3] dist|flag, h[4] lb, h[5] ub
+        uint32_t h[6];
+#pragma unroll
+        for (int i = 0; i < 6; ++i) h[i] = c1 ? v[1][i + 2] : v[0][i + 2];
+        const uint32_t r_unitig = h[0], r_ec = h[2];
+        const bool r_strand = (is_canon == ((h[3] >> 31) != 0));
+        const ReadView rv = view(c, l);
+        int ns = s, np_ = pc, npr = P_BUILD;     // the chain's next state, position and key preparation
         bool push = false, end_chain = false, to_backoff = false;
         int nv_from = -1;      // >= 0: continue with p = next_valid(nv_from) in MAIN (or BACKOFF)
-        if (st[c] == S_MAIN) {
-          if (!f) {
-            nv_from = p[c] + 1;
+        if (s == S_MAIN) {
+          if (!fc) {
+            nv_from = pc + 1;
           } else {
             push = true;
-            const int r_dist = (int)(v[c][5] & 0x7FFFFFFFu);
-            const int off = r_dist - (int)v[c][6], blen = (int)(v[c][7] - v[c][6]);
+            const int r_dist = (int)(h[3] & 0x7FFFFFFFu);
+            const int off = r_dist - (int)h[4], blen = (int)(h[5] - h[4]);
             const int dist = r_strand ? (blen - 1 - off) : off;               // 1780-1788
             if (dist >= 2) {
-              const int np = (p[c] + dist >= l - k) ? (l - k) : (p[c] + dist);   // 1793-1798
+              const int np = (pc + dist >= l - k) ? (l - k) : (pc + dist);      // 1793-1798
               const int p2 = rv.next_valid(np);                               // kit2 += nextPos-pos (adv 0: p itself)
               if (p2 < 0) {
                 end_chain = true;                                           // 1882-1886
@@ -729,34 +785,33 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
                 cw(C_P2, c) = (uint32_t)p2;
                 cw(C_DIST, c) = (uint32_t)dist;
                 cw(C_HU, c) = r_unitig; cw(C_HE, c) = r_ec;
-                st[c] = S_JUMP;
-                need_prep[c] = true;
+                ns = S_JUMP;
               }
             } else {
-              nv_from = p[c] + 1;
+              nv_from = pc + 1;
             }
           }
-        } else if (st[c] == S_JUMP) {
-          const bool found2 = !f || (cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec);   // 1807-1815
+        } else if (s == S_JUMP) {
+          const bool found2 = !fc || (cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec);   // 1807-1815
           const int dist = (int)cw(C_DIST, c);
-          const int found2pos = !f ? p[c] : p[c] + dist;
+          const int found2pos = !fc ? pc : pc + dist;
           if (found2) {
             if (found2pos >= l - k) end_chain = true;                       // "fake position", break (1819-1822)
             else nv_from = (int)cw(C_P2, c) + 1;                            // kit = kit2; ++kit
           } else {
             cw(C_H2U, c) = r_unitig; cw(C_H2E, c) = r_ec;
             if (dist > 4) {
-              const int middlePos = (p[c] + (int)cw(C_NP, c)) / 2;
+              const int middlePos = (pc + (int)cw(C_NP, c)) / 2;
               const int p3 = rv.next_valid(middlePos);                      // kit3 += middlePos-pos
-              if (p3 >= 0) { cw(C_P3, c) = (uint32_t)p3; st[c] = S_MIDDLE; need_prep[c] = true; }
+              if (p3 >= 0) { cw(C_P3, c) = (uint32_t)p3; ns = S_MIDDLE; }
               else to_backoff = true;
             } else {
               to_backoff = true;
             }
           }
-        } else if (st[c] == S_MIDDLE) {
-          const bool foundMiddle = f && ((cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec) ||
-                                         (cw(C_H2U, c) == r_unitig && cw(C_H2E, c) == r_ec));
+        } else if (s == S_MIDDLE) {
+          const bool foundMiddle = fc && ((cw(C_HU, c) == r_unitig && cw(C_HE, c) == r_ec) ||
+                                          (cw(C_H2U, c) == r_unitig && cw(C_H2E, c) == r_ec));
           if (foundMiddle) {
             push = true;
             if ((int)cw(C_NP, c) >= l - k) end_chain = true;               // 1867
@@ -765,18 +820,18 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             to_backoff = true;
           }
         } else {   // S_BACKOFF: the single probe of the back-off loop
-          push = f;
-          nv_from = p[c] + 1;
+          push = fc;
+          nv_from = pc + 1;
         }
         if (push) {
-          if (!hv[c]) {
-            hv[c] = true;   // only a MAIN hit can be the first hit of a read
-            cw(C_BLK, c) = v[c][3];
-            cw(C_DS, c) = (v[c][5] & 0x7FFFFFFFu) | (r_strand ? 0x80000000u : 0u);
-            cw(C_POS, c) = (uint32_t)p[c];
+          if (!((hv >> c) & 1u)) {
+            hv |= 1u << c;   // only a MAIN hit can be the first hit of a read
+            cw(C_BLK, c) = h[1];
+            cw(C_DS, c) = (h[3] & 0x7FFFFFFFu) | (r_strand ? 0x80000000u : 0u);
+            cw(C_POS, c) = (uint32_t)pc;
           }
           if (r_ec != ba.empty_ec) {               // "Don't intersect empty EC", MinCollector.cpp:468-469
-            hs[c] = true;
+            hs |= 1u << c;
             // the tuple is shared by both chains: a handle the other chain pushed (also in this iteration) is a duplicate
             bool dup = false;
             const int n_sh = n_e < KB_MAX_E ? n_e : KB_MAX_E;
@@ -789,23 +844,31 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             }
           }
         }
-        if (to_backoff) nv_from = p[c] + 1;        // ++kit; backOff = true
+        if (to_backoff) nv_from = pc + 1;          // ++kit; backOff = true
         if (nv_from >= 0) {
-          p[c] = rv.next_valid(nv_from);
-          if (p[c] < 0) end_chain = true;
-          else { st[c] = to_backoff ? S_BACKOFF : S_MAIN; need_prep[c] = true; }
+          // where the k-mer the chain holds starts: the next one is rolled from it when it starts one base later
+          const int key_pos = (s == S_MAIN || s == S_BACKOFF) ? pc : (int)cw(s == S_JUMP ? C_P2 : C_P3, c);
+          np_ = rv.next_valid(nv_from);
+          if (np_ < 0) end_chain = true;
+          else { ns = to_backoff ? S_BACKOFF : S_MAIN; npr = np_ == key_pos + 1 ? P_ROLL : P_BUILD; }
         }
-        if (end_chain) st[c] = S_FIN;
-        KB_MS_ONLY(if (st[c] == S_FIN) end_run(c);)
+        if (end_chain) ns = S_FIN;
+        KB_MS_ONLY(if (ns == S_FIN) end_run(c);)
+        if (c1) { st[1] = ns; p[1] = np_; prep[1] = npr; }
+        else { st[0] = ns; p[0] = np_; prep[0] = npr; }
       }
     }
+#ifdef KB_MATCH_STATS
+    KB_MS(MS_GEN_PASSES, __reduce_max_sync(0xFFFFFFFFu, n_pass));   // the warp's passes of the general transition
+#endif
   }
   // statistics: lookups, slot visits, memo hits (every warp leaves the loop with all its fragments finalised)
   __syncthreads();
   if (tid < 3 && s_tot[tid]) atomicAdd(&dd.stats[tid == 0 ? 0 : (tid == 1 ? 3 : 2)], s_tot[tid]);
 #ifdef KB_MATCH_STATS
   for (int i = 0; i < MS_N; ++i) {
-    const bool per_warp = i == MS_WARP_ITERS || i == MS_SERVICE_ROUNDS || i == MS_CYCLES_LOOKUP || i == MS_CYCLES_SERVICE;
+    const bool per_warp = i == MS_WARP_ITERS || i == MS_SERVICE_ROUNDS || i == MS_CYCLES_LOOKUP || i == MS_CYCLES_SERVICE ||
+                          i == MS_GEN_PASSES;
     unsigned long long x = ms[i];
     if (!per_warp)
       for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xFFFFFFFFu, x, o);

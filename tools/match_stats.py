@@ -2,6 +2,9 @@
 """Where match_kernel's iterations go, on the benchmark workload: builds the library with -DKB_MATCH_STATS into a
 temporary directory (the in-tree build is untouched), runs the benchmark batches once and prints one JSON line with
 the summed per-launch counters and their shares.  The counters slow the kernel, so its times are not reported; the counts themselves do not depend on that.
+Of the chain iterations (a live chain's probes, collisions included), the share settled on the straight-line path
+(collisions, MAIN misses on mates without N) is reported, and the passes of the general transition per warp-iteration
+(a warp runs as many as its busiest lane needs).
 The clock split of a lookup iteration (keys and hashes / the wait for the filter and slot loads / the state transitions)
 is given in cycles per lane-iteration.  KB_NVCC_DEFS adds defines to the build (e.g. -DKB_MATCH_MIN_BLOCKS=4); a
 library built beforehand with -DKB_MATCH_STATS (and those defines) can be named by KB_LIB_PATH instead."""
@@ -68,6 +71,8 @@ def run(tmp):
            "share_main_miss_of_lookups": main_miss / max(1, st["n_probes"]),
            "share_main_miss_of_chain_iters": main_miss / lane,
            "live_chains_per_warp_iter": tot["chain_iters"] / max(1, tot["warp_iters"]),
+           "share_straight_of_chain_iters": tot["straight"] / lane,
+           "general_passes_per_warp_iter": tot["gen_passes"] / max(1, tot["warp_iters"]),
            "service_share_of_cycles": tot["cycles_service"] / max(1, tot["cycles_service"] + tot["cycles_lookup"]),
            "cycles_per_warp_iter": tot["cycles_lookup"] / max(1, tot["warp_iters"]),
            "cycles_per_lane_iter": {p: tot["cycles_" + p] / max(1, tot["lane_iters"]) for p in ("key", "wait", "step")},
