@@ -100,7 +100,7 @@ EXPORTED_SYMBOLS = [
     "kb_quant_get_timings", "kb_quant_finalize", "kb_quant_ec_table", "kb_quant_get_flens",
     "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_read_priors", "kb_em_set_priors", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
     "kb_comm_unique_id", "kb_comm_create", "kb_comm_create_from_nccl", "kb_comm_create_all", "kb_comm_reserve", "kb_comm_free",
-    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_run_priors", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_lengths", "kb_bus_set_aa", "kb_bus_frame_clashes", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
+    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_run_priors", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_set_batch_barcodes", "kb_bus_lengths", "kb_bus_set_aa", "kb_bus_frame_clashes", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
 ]
 
 # kb_tcc_bootstrap_cb: (user, first problem, count, est_counts, rounds, resampled counts or NULL) -> 0 to go on
@@ -180,6 +180,7 @@ def lib():
     L.kb_bus_batch_device.argtypes = [vp, vp, vp, u32, u32, C.POINTER(u32), C.POINTER(vp)]
     L.kb_bus_lengths.argtypes = [vp, vp, vp]
     L.kb_bus_begin_sample.argtypes = [vp, C.c_uint64]
+    L.kb_bus_set_batch_barcodes.argtypes = [vp, C.c_int32]
     L.kb_bus_set_aa.argtypes = [vp, C.c_int32]
     L.kb_bus_frame_clashes.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.kb_fastx_summary.argtypes = [C.c_char_p, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
@@ -460,8 +461,10 @@ class Comm:
 class BUSProcessor(MinCollector):
     """`kallisto bus` run (BUSProcessor::processBuffer + the BUS part of MasterProcessor::update)."""
 
-    def __init__(self, index, technology, strand="default", num=False, max_batch_sets=0, tag=None, aa=False):
-        """aa: `bus --aa`, the reads translated in six frames against an index built with `kallisto index --aa`."""
+    def __init__(self, index, technology, strand="default", num=False, max_batch_sets=0, tag=None, aa=False,
+                 batch_barcodes=False):
+        """aa: `bus --aa`, the reads translated in six frames against an index built with `kallisto index --aa`.
+        batch_barcodes: `bus --batch --batch-barcodes`, the sample of begin_sample in front of every barcode."""
         self.index = index
         self.paired = False
         tech = TECHNOLOGIES[technology.upper()] if isinstance(technology, str) else technology
@@ -490,6 +493,8 @@ class BUSProcessor(MinCollector):
         self._stats = None
         if aa:
             _ck(lib().kb_bus_set_aa(self._h, 1))
+        if batch_barcodes:
+            _ck(lib().kb_bus_set_batch_barcodes(self._h, 1))
 
     def process_sets(self, files):
         """files: list of (bases uint8, offsets uint32) per file of the technology -> structured record array."""
@@ -516,7 +521,8 @@ class BUSProcessor(MinCollector):
         return nrec.value, drec.value
 
     def begin_sample(self, barcode):
-        """Batch mode (`bus -x BULK`): the following read sets belong to the sample with this fake barcode."""
+        """Batch mode (`bus -x BULK` / `--batch`): the following read sets belong to this sample: the fake barcode without
+        a barcode read, the prefix of batch_barcodes with one; fragment lengths and --num read numbers start again."""
         _ck(lib().kb_bus_begin_sample(self._h, C.c_uint64(barcode)))
 
     def lengths(self):

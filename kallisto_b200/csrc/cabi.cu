@@ -634,6 +634,11 @@ int kb_bus_begin_sample(kb_quant* q, uint64_t barcode) {
   return guarded([&] { q->q->bus_begin_sample(barcode); });
 }
 
+int kb_bus_set_batch_barcodes(kb_quant* q, int32_t on) {
+  if (!q) return fail(KB_ERR_INVALID, "kb_bus_set_batch_barcodes: null argument");
+  return guarded([&] { q->q->set_batch_barcodes(on != 0); });
+}
+
 int kb_bus_lengths(kb_quant* q, uint32_t* bc_hist, uint32_t* umi_hist) {
   if (!q || !bc_hist || !umi_hist) return fail(KB_ERR_INVALID, "kb_bus_lengths: null argument");
   return guarded([&] { q->q->bus_lengths(bc_hist, umi_hist); });

@@ -754,7 +754,7 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   if (sp.tag_len) grow(bus_notag_, n1);
   grow(bus_isnew_, n1); grow(bus_newrank_, n1); grow(bus_ismapped_, n1); grow(bus_rank_, n1); grow(bus_rec_, n1);
   if (bus_hist_.n < 66) { bus_hist_.alloc(66); bus_hist_.zero(st); }
-  bus_nvalid_.grow(1);
+  bus_nvalid_.grow(2);      // [0] valid read sets, [1] --batch-barcodes sets with more than 32 barcode letters
   if (bus_idof_.n < ix_.dict_cap) { bus_idof_.alloc(ix_.dict_cap); launch_fill_i32(bus_idof_.p, ix_.dict_cap, -1, st); }
   const size_t tb = bus_scan_bytes(n_sets);
   if (bus_tmp_.n < tb) bus_tmp_.alloc(std::max(tb, bus_scan_bytes(opt_.max_batch_reads)));
@@ -764,7 +764,7 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   a.spec = sp;
   a.barcode = (uint64_t*)bus_bc_.p; a.umi = (uint64_t*)bus_umi_.p; a.flags = bus_flags_.p; a.skip = bus_skip_.p;
   a.notag = sp.tag_len ? bus_notag_.p : nullptr;
-  a.bc_hist = bus_hist_.p; a.umi_hist = bus_hist_.p + 33; a.n_valid = bus_nvalid_.p;
+  a.bc_hist = bus_hist_.p; a.umi_hist = bus_hist_.p + 33; a.n_valid = bus_nvalid_.p; a.n_long_bc = bus_nvalid_.p + 1;
   launch_bus_fields(a, st);
   KB_CK(cudaGetLastError());
   // the cDNA read(s): single-read or paired pseudoalignment with the strand filter of the technology
@@ -833,25 +833,45 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   KB_CK(cudaGetLastError());
   n_kernel_launches += 4;      // bus_fields, bus_newflag, bus_newid, bus_records (CUB scans not counted)
   uint32_t n_new = 0, n_rec = 0;
-  unsigned long long n_valid = 0;
+  unsigned long long n_valid[2] = {0, 0};
   bus_newrank_.download(&n_new, 1, n_sets, st);
   bus_rank_.download(&n_rec, 1, n_sets, st);
-  bus_nvalid_.download(&n_valid, 1, 0, st);
+  bus_nvalid_.download(n_valid, 2, 0, st);
   KB_CK(cudaStreamSynchronize(st));
+  if (n_valid[1])
+    throw Error("kallisto_b200: --batch-barcodes: " + std::to_string(n_valid[1]) + " read set(s) of this batch have a barcode of "
+                "more than 32 letters, which cannot take the sample's number in front of it");
   bus_next_id_ += n_new;
-  bus_valid_total_ += n_valid;
+  bus_valid_total_ += n_valid[0];
   return n_rec;
 }
 
 void Quant::bus_begin_sample(uint64_t barcode) {
   if (!opt_.bus) throw Error("kallisto_b200: not a bus run");
-  if (opt_.bus_spec.n_bc != 0) throw Error("kallisto_b200: sample barcodes need a technology without a barcode read");
-  opt_.bus_spec.fake_bc = barcode;
+  if (opt_.bus_spec.n_bc == 0) opt_.bus_spec.fake_bc = barcode;
+  else opt_.bus_spec.bc_prefix = barcode;      // in front of the barcode only with --batch-barcodes (batch_bc)
   bus_sample_base_ = n_frag_total_;
   // per-sample fragment-length histogram and quota (batchFlens[id] / tlencounts[id], src/ProcessReads.cpp:486-493)
   std::fill(flens_.begin(), flens_.end(), 0u);
   tl_list_.clear();
   tlencount_ = 0;
+}
+
+void Quant::set_batch_barcodes(bool on) {
+  if (!opt_.bus) throw Error("kallisto_b200: --batch-barcodes needs a bus run");
+  if (n_frag_total_ != 0) throw Error("kallisto_b200: --batch-barcodes must be chosen before the first batch");
+  const BusSpec& sp = opt_.bus_spec;
+  if (on && sp.n_bc > 0) {
+    int fixed = 0;      // letters of the pieces with a stop; a piece to the end of its read adds to them
+    for (int p = 0; p < sp.n_bc; ++p)
+      if (sp.bc_b[p] != 0) fixed += sp.bc_b[p] - sp.bc_a[p];
+    // the reference forms a barcode of 32 - blen batch letters there, with 32 - blen wrapped around (size_t)
+    if (fixed > 32)
+      throw Error("kallisto_b200: --batch-barcodes needs a barcode of at most 32 letters; the technology's has " +
+                  std::to_string(fixed));
+  }
+  // a technology without a barcode read takes the sample's number as its barcode (kb_bus_begin_sample) either way
+  opt_.bus_spec.batch_bc = (on && sp.n_bc > 0) ? 1 : 0;
 }
 
 void Quant::set_aa(bool on) {

@@ -322,6 +322,8 @@ struct BusSpec {        // BUSOptions (src/common.h:38-91): where barcode / UMI 
   unsigned long long fake_bc;   // n_bc == 0: the barcode every record gets (0 = 16 x 'A'; batch mode: the sample's id, :1603-1607)
   int tag_len;                  // --tag: length of the tag sequence that precedes the UMI (0 = none); umi_a[0] is already advanced by it
   unsigned long long tag_bin;   // stringToBinary(tag)
+  int batch_bc;                 // --batch-barcodes with a barcode read: the sample's number goes in front of the barcode
+  unsigned long long bc_prefix; // batch_bc: the sample's number (batch_id_mapping[id], src/ProcessReads.cpp:1617-1626)
 };
 struct BusArgs {
   const uint8_t* bases[4];
@@ -337,6 +339,7 @@ struct BusArgs {
   uint32_t* bc_hist;    // 33 bins
   uint32_t* umi_hist;   // 33 bins
   unsigned long long* n_valid;
+  unsigned long long* n_long_bc;   // batch_bc: read sets whose barcode has more than 32 letters (the run must stop)
 };
 size_t bus_scan_bytes(uint32_t n);
 void launch_bus_fields(const BusArgs& a, cudaStream_t st);

@@ -99,11 +99,20 @@ __global__ void __launch_bounds__(256) bus_fields_kernel(BusArgs a) {
       }
       if (ok) {
         if (b.n <= 32) atomicAdd(&a.bc_hist[b.n], 1u);
+        uint32_t bf = b.flag();
+        if (sp.batch_bc) {
+          // --batch-barcodes (:1617-1626): binaryToString(batch, 32 - blen) + binaryToString(stringToBinary(bc), blen),
+          // re-encoded: 32 letters with the sample's number in front, an N already turned into G, so no N flag.  Past
+          // 32 letters the reference's 32 - blen wraps around; such a set stops the run on the host instead.
+          if (b.n > 32) atomicAdd(a.n_long_bc, 1ull);
+          else if (b.n < 32) b.r |= (sp.bc_prefix & ((1ull << (64 - 2 * b.n)) - 1)) << (2 * b.n);
+          bf = 0;
+        }
         a.barcode[i] = b.r;
         a.umi[i] = u.r;
         // without a UMI stringToBinary runs once only, so the UMI half of the flags repeats the barcode's (:1736-1743)
-        const uint32_t uf = (sp.no_umi || sp.tag_len) ? b.flag() : u.flag();
-        a.flags[i] = sp.num_flag ? (uint32_t)(a.set_base + i) : (b.flag() | (uf << 8));
+        const uint32_t uf = (sp.no_umi || sp.tag_len) ? bf : u.flag();
+        a.flags[i] = sp.num_flag ? (uint32_t)(a.set_base + i) : (bf | (uf << 8));
         valid = true;
       }
     }
