@@ -94,7 +94,9 @@ int kb_pseudoalign_batch_pe(kb_quant* q, const char* bases1, const uint32_t* off
  * full PCIe speed without the caller linking against CUDA). */
 void* kb_host_alloc(size_t bytes);
 void kb_host_free(void* p);
-/* Same with DEVICE pointers (inputs already resident in HBM); asynchronous on the run's stream. */
+/* Same with DEVICE pointers (inputs already resident in HBM); asynchronous on the run's stream.  The kernels run on
+ * the run's internal streams, two batches at a time; the run's stream waits only until the inputs have been read, so
+ * the caller may overwrite them in that stream's order.  Everything that reads results waits for the batches. */
 int kb_pseudoalign_batch_device(kb_quant* q, const void* d_bases, const uint32_t* d_offsets, uint32_t n_reads,
                                 uint32_t fixed_len, uint32_t max_read_len);
 int kb_quant_sync(kb_quant* q);

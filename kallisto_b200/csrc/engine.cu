@@ -293,7 +293,11 @@ Quant::Quant(Index& ix, const QuantOptions& opt) : ix_(ix), opt_(opt), flens_(10
   for (int i = 0; i < 2; ++i) {
     KB_CK(cudaEventCreateWithFlags(&ev_copied_[i], cudaEventDisableTiming));
     KB_CK(cudaEventCreateWithFlags(&ev_done_[i], cudaEventDisableTiming));
+    KB_CK(cudaStreamCreateWithFlags(&bstream_[i], cudaStreamNonBlocking));
+    KB_CK(cudaEventCreateWithFlags(&ev_packed_[i], cudaEventDisableTiming));
+    KB_CK(cudaEventCreateWithFlags(&ev_last_[i], cudaEventDisableTiming));
   }
+  KB_CK(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
   cudaStream_t st = stream_;
   apply_l2_window();
   const uint64_t nE = ix_.flat.n_ec();
@@ -339,34 +343,33 @@ Quant::Quant(Index& ix, const QuantOptions& opt) : ix_(ix), opt_(opt), flens_(10
   dd_.tpool = tpool_.p; dd_.tpool_top = counters_.p + 16; dd_.tpool_cap = tpool_cap;
   dd_.error = error_.p; dd_.stats = counters_.p + 32;
 
-  // batch staging
+  // batch work buffers, both slots (BatchSlot)
   const uint32_t max_frag = opt_.max_batch_reads;
-  bws_->d_handles.grow(max_frag);
-  bws_->d_tl.grow(max_frag);
-  bws_->d_qcount.grow(1);
-  bws_->d_qentries.grow((size_t)max_frag * KB_Q_STRIDE);
-  // rare path: fragments with more than KB_MAX_E distinct EC sets (spill area per resident lane + wide queue)
-  bws_->d_qbig_count.grow(1);
-  bws_->d_qbig.grow((size_t)KB_QBIG_CAP * KB_QBIG_STRIDE);
-  {
-    int sms = 0, tpsm = 0;
-    KB_CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ix_.device));
-    KB_CK(cudaDeviceGetAttribute(&tpsm, cudaDevAttrMaxThreadsPerMultiProcessor, ix_.device));
-    const size_t lanes = (size_t)sms * (size_t)tpsm;
-    bws_->d_spill.grow(lanes * KB_SPILL);
+  int sms = 0, tpsm = 0;
+  KB_CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ix_.device));
+  KB_CK(cudaDeviceGetAttribute(&tpsm, cudaDevAttrMaxThreadsPerMultiProcessor, ix_.device));
+  for (BatchSlot& w : bws_->slot) {
+    w.d_handles.grow(max_frag);
+    w.d_tl.grow(max_frag);
+    w.d_counters.grow(KB_BATCH_COUNTER_WORDS);
+    w.d_qentries.grow((size_t)max_frag * KB_Q_STRIDE);
+    w.d_rlen.grow(2 * (size_t)max_frag);
+    // rare path: fragments with more than KB_MAX_E distinct EC sets (spill area per resident lane + wide queue)
+    w.d_qbig.grow((size_t)KB_QBIG_CAP * KB_QBIG_STRIDE);
+    w.d_spill.grow((size_t)sms * (size_t)tpsm * KB_SPILL);
   }
-  // resolve-kernel scratch: 2 x max_set_len words per lane group, at most ~1 GiB in total
+  // resolve-kernel scratch: 2 x max_set_len words per lane group, at most ~0.5 GiB per slot
   {
     const char* e = getenv("KB_RESOLVE_G");
     const int g = e ? atoi(e) : 32;
     resolve_group_ = (g == 4 || g == 8 || g == 16 || g == 32) ? (uint32_t)g : 32u;
   }
   const uint64_t stride = std::max<uint64_t>(64, 2ull * ix_.max_set_len);
-  uint64_t warps = (1ull << 28) / stride;
+  uint64_t warps = (1ull << 27) / stride;
   // the kernel is latency-bound: fill the SMs (32 warps each), every warp split into 32 / group lane groups
   warps = std::min<uint64_t>((uint64_t)device_sm_count() * 32 * (32 / resolve_group_), std::max<uint64_t>(64, warps));
   n_resolve_warps_ = (uint32_t)(warps / 16 * 16);
-  bws_->d_scratch.grow((size_t)n_resolve_warps_ * stride);
+  for (BatchSlot& w : bws_->slot) w.d_scratch.grow((size_t)n_resolve_warps_ * stride);
   scratch_stride_ = (uint32_t)stride;
   // EM workspace: sized once per index for the EC tables runs on it normally end with (twice the index's own sets),
   // so that the timed EM tail of a run does not allocate; it still grows on demand
@@ -430,6 +433,8 @@ EmCompWs EmWs::comp(uint32_t T, uint32_t R, size_t nnz, int max_iter, const doub
 }
 
 Quant::~Quant() {
+  for (cudaStream_t b : bstream_)
+    if (b) cudaStreamSynchronize(b);
   if (stream_) cudaStreamSynchronize(stream_);
   if (own_ws_) { delete emws_; delete bws_; } else { ix_.ws_in_use = false; }
   if (h_off_pinned_) cudaFreeHost(h_off_pinned_);
@@ -438,11 +443,18 @@ Quant::~Quant() {
     if (ev_copied_[i]) cudaEventDestroy(ev_copied_[i]);
     if (ev_done_[i]) cudaEventDestroy(ev_done_[i]);
   }
+  for (int i = 0; i < 2; ++i) {
+    if (ev_packed_[i]) cudaEventDestroy(ev_packed_[i]);
+    if (ev_last_[i]) cudaEventDestroy(ev_last_[i]);
+    if (bstream_[i]) cudaStreamDestroy(bstream_[i]);
+  }
+  if (ev_fork_) cudaEventDestroy(ev_fork_);
   if (copy_stream_) cudaStreamDestroy(copy_stream_);
   if (stream_ && own_stream_) cudaStreamDestroy(stream_);
 }
 
 void Quant::set_stream(cudaStream_t st) {
+  join();
   KB_CK(cudaStreamSynchronize(stream_));
   if (stream_ && own_stream_) cudaStreamDestroy(stream_);
   stream_ = st;
@@ -450,7 +462,8 @@ void Quant::set_stream(cudaStream_t st) {
   apply_l2_window();
 }
 
-// Kernels launched on the run's stream treat the presence filter as persisting in L2; everything else streams.
+// Kernels launched on the run's streams treat the presence filter as persisting in L2; everything else streams.  The
+// window is a stream attribute: match_kernel runs on the internal streams, so they carry it too.
 void Quant::apply_l2_window() {
   if (!ix_.filter.p || ix_.l2_persist_bytes == 0) return;
   int max_win = 0;
@@ -463,12 +476,15 @@ void Quant::apply_l2_window() {
   v.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)ix_.l2_persist_bytes / (double)bytes);
   v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
   v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-  if (cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
+  for (cudaStream_t s : {stream_, bstream_[0], bstream_[1]})
+    if (cudaStreamSetAttribute(s, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
 }
 
 Quant::Timings Quant::timings() {
+  join();
   KB_CK(cudaStreamSynchronize(stream_));
   for (size_t i = 0; i + 3 < events_.size(); i += 4) {
+    // with batches overlapping, each is a span on its own stream that other batches' kernels may share
     float a = 0, b = 0, c = 0;
     KB_CK(cudaEventElapsedTime(&c, events_[i], events_[i + 1]));
     KB_CK(cudaEventElapsedTime(&a, events_[i + 1], events_[i + 2]));
@@ -484,9 +500,19 @@ Quant::Timings Quant::timings() {
   return tacc_;
 }
 
-void Quant::sync() { KB_CK(cudaStreamSynchronize(stream_)); }
+void Quant::sync() {
+  join();
+  KB_CK(cudaStreamSynchronize(stream_));
+}
+
+void Quant::join() {
+  if (!pending_) return;
+  for (cudaEvent_t e : ev_last_) KB_CK(cudaStreamWaitEvent(stream_, e, 0));
+  pending_ = false;
+}
 
 void Quant::check_device_errors() {
+  join();
   int herr = 0;
   error_.download(&herr, 1, 0, stream_);
   KB_CK(cudaStreamSynchronize(stream_));
@@ -504,8 +530,18 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
                       uint32_t max_read_len, const uint8_t* d_bases2, const uint32_t* d_off2) {
   const uint32_t n_frag = opt_.paired ? n_reads / 2 : n_reads;
   if (opt_.paired && (n_reads & 1)) throw Error("kallisto_b200: odd number of reads in a paired batch");
-  if (n_frag > bws_->d_handles.n) throw Error("kallisto_b200: batch larger than max_batch_reads");
+  const int b = (int)(n_batches_ & 1);
+  BatchSlot& w = bws_->slot[b];
+  if (n_frag > w.d_handles.n) throw Error("kallisto_b200: batch larger than max_batch_reads");
   if (n_frag == 0) return;
+  // the batch runs on internal stream b, after what the caller enqueued on the run's stream so far; stream b last ran
+  // batch i - 2, the one that used these buffers before
+  const cudaStream_t bs = bstream_[b];
+  ++n_batches_;
+  last_slot_ = b;
+  pending_ = true;
+  KB_CK(cudaEventRecord(ev_fork_, stream_));
+  KB_CK(cudaStreamWaitEvent(bs, ev_fork_, 0));
   ecs_valid_ = false;
   dev_stats_valid_ = false;
   dev_problem_valid_ = false;
@@ -520,14 +556,15 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ba.strand_mode = aa_ ? 0 : opt_.strand_mode;     // --aa: the frames are matched unstranded, cfc_select_kernel filters the set
   ba.frag_base = have_frag_base_ ? frag_base_ : n_frag_total_;
   have_frag_base_ = false;
-  ba.handle_out = bws_->d_handles.p;
+  ba.handle_out = w.d_handles.p;
   const bool want_fld = opt_.paired && opt_.collect_fld && tlencount_ < 10000;   // ProcessReads.cpp:981-1017
-  ba.tl_out = want_fld ? bws_->d_tl.p : nullptr;
-  ba.q_count = bws_->d_qcount.p;
-  ba.q_entries = bws_->d_qentries.p;
-  ba.spill = bws_->d_spill.p;
-  ba.qbig_count = bws_->d_qbig_count.p;
-  ba.qbig_entries = bws_->d_qbig.p;
+  ba.tl_out = want_fld ? w.d_tl.p : nullptr;
+  ba.q_count = w.d_counters.p;
+  ba.qbig_count = w.d_counters.p + KB_BATCH_COUNTER_LINE;
+  ba.take = w.d_counters.p + 2 * KB_BATCH_COUNTER_LINE;
+  ba.q_entries = w.d_qentries.p;
+  ba.spill = w.d_spill.p;
+  ba.qbig_entries = w.d_qbig.p;
   ba.qbig_cap = KB_QBIG_CAP;
   ba.nb = std::max<uint32_t>(1, (max_read_len + 31) / 32);
   ba.pstride = (3 * ba.nb + 7) & ~7u;
@@ -535,9 +572,11 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
     const size_t need = (size_t)n_reads * ba.pstride;
     if ((uint64_t)n_reads * ba.nb >= (1ull << 32))      // pack_kernel / dlist_scan_kernel index (read, word) with 32 bits
       throw Error("kallisto_b200: batch too large for its longest read (reads x ceil(max length / 32) must be < 2^32)");
-    if (bws_->d_packed.n < need) bws_->d_packed.alloc(std::max(need, (size_t)opt_.max_batch_reads * 2 * 16));
+    if (w.d_packed.n < need) w.d_packed.alloc(std::max(need, (size_t)opt_.max_batch_reads * 2 * 16));
+    if (w.d_rlen.n < n_reads) w.d_rlen.alloc(n_reads);
   }
-  ba.packed = bws_->d_packed.p;
+  ba.packed = w.d_packed.p;
+  ba.rlen = w.d_rlen.p;
   ba.empty_ec = ix_.empty_ec;
   ba.refill_min = opt_.refill_min;
   ba.skip = cur_skip_;
@@ -547,9 +586,9 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
     if (cur_skip_) {
       ba.skip_w = const_cast<uint8_t*>(cur_skip_);          // bus: the scan adds to the bad-barcode marks
     } else {
-      if (bws_->d_skip.n < n_frag) bws_->d_skip.alloc(std::max<size_t>(n_frag, opt_.max_batch_reads));
-      KB_CK(cudaMemsetAsync(bws_->d_skip.p, 0, n_frag, stream_));
-      ba.skip = ba.skip_w = bws_->d_skip.p;
+      if (w.d_skip.n < n_frag) w.d_skip.alloc(std::max<size_t>(n_frag, opt_.max_batch_reads));
+      KB_CK(cudaMemsetAsync(w.d_skip.p, 0, n_frag, bs));
+      ba.skip = ba.skip_w = w.d_skip.p;
     }
   }
   ba.fp_fl = opt_.fp_fl;
@@ -561,7 +600,7 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ba.no_count = aa_ ? 1 : 0;
   ba.first_hit = aa_ ? cfc_first_.p : nullptr;
   ResolveArgs ra{};
-  ra.scratch = bws_->d_scratch.p;
+  ra.scratch = w.d_scratch.p;
   ra.scratch_stride = scratch_stride_;
   ra.n_warps = n_resolve_warps_;
   ra.group = resolve_group_;
@@ -577,20 +616,23 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
     for (int i = 0; i < 4; ++i) KB_CK(cudaEventCreate(&events_[base + i]));
     ev = events_.data() + base;
   }
-  launch_pseudoalign(ix_.dev, dd_, ba, ra, tpb, stream_, ev);
+  launch_pseudoalign(ix_.dev, dd_, ba, ra, tpb, bs, ev, ev_packed_[b]);
   KB_CK(cudaGetLastError());
+  // the caller may overwrite its input in its stream order once pack_kernel (and dlist_scan_kernel) have read it
+  KB_CK(cudaStreamWaitEvent(stream_, ev_packed_[b], 0));
   n_kernel_launches += 3 + (ba.skip_w ? 1 : 0);   // pack_kernel, [dlist_scan_kernel,] match_kernel, resolve_kernel
   if (aa_) {
-    launch_cfc_select(ix_.dev, dd_, ba, ra, n_frag / 6, opt_.strand_mode, cfc_handles_.p, cfc_clashes_.p, stream_);
+    launch_cfc_select(ix_.dev, dd_, ba, ra, n_frag / 6, opt_.strand_mode, cfc_handles_.p, cfc_clashes_.p, bs);
     KB_CK(cudaGetLastError());
     ++n_kernel_launches;
   }
+  if (want_fld) launch_fld_finalize(dd_, ba, bs);
+  KB_CK(cudaEventRecord(ev_last_[b], bs));
   if (want_fld) {
-    launch_fld_finalize(dd_, ba, stream_);
     ++n_kernel_launches;
     h_tl_.resize(n_frag);
-    bws_->d_tl.download(h_tl_.data(), n_frag, 0, stream_);
-    KB_CK(cudaStreamSynchronize(stream_));
+    w.d_tl.download(h_tl_.data(), n_frag, 0, bs);
+    KB_CK(cudaStreamSynchronize(bs));
     // first (10000 - tlencount) qualifying fragments of this batch, in read order
     int goal = 10000 - (int)tlencount_;
     uint32_t local = 0;
@@ -641,7 +683,8 @@ void Quant::pseudoalign_host(const char* bases, const uint32_t* off, uint32_t n_
   KB_CK(cudaEventRecord(ev_done_[s], stream_));
   if (handles_out) {
     const uint32_t n_frag = opt_.paired ? n_reads / 2 : n_reads;
-    bws_->d_handles.download(handles_out, n_frag, 0, stream_);
+    join();
+    bws_->slot[last_slot_].d_handles.download(handles_out, n_frag, 0, stream_);
     KB_CK(cudaStreamSynchronize(stream_));
   } else {
     // the caller may reuse its buffers once the copy is done; the kernels keep running
@@ -688,7 +731,8 @@ void Quant::pseudoalign_host_pe(const char* bases1, const uint32_t* off1, const 
   run_batch(b1.p, off1 ? o1.p : nullptr, 2 * n_pairs, fixed_len, maxlen, b2.p, off1 ? o2.p : nullptr);
   KB_CK(cudaEventRecord(ev_done_[s], stream_));
   if (handles_out) {
-    bws_->d_handles.download(handles_out, n_pairs, 0, stream_);
+    join();
+    bws_->slot[last_slot_].d_handles.download(handles_out, n_pairs, 0, stream_);
     KB_CK(cudaStreamSynchronize(stream_));
   } else {
     KB_CK(cudaEventSynchronize(ev_copied_[s]));
@@ -780,7 +824,6 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   }
   maxlen = maxlen > min_start ? maxlen - min_start : 1;
   const uint64_t base = n_frag_total_;
-  const int32_t* handles = bws_->d_handles.p;
   cur_skip_ = bus_skip_.p;
   cur_start_ = (uint32_t)sp.seq_start;
   if (aa_) {
@@ -813,7 +856,6 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
     cur_skip_ = nullptr;
     cur_start_ = 0;
     run_batch(cfc_b_.p, cfc_o_.p, 6 * n_sets, 0, maxlen);
-    handles = cfc_handles_.p;
   } else if (sp.paired) {
     // two sequence reads (busopt.paired, src/ProcessReads.cpp:1550-1567,1646-1650): the pair goes through the same
     // match x 2 / intersectKmers / strand filter / mapPair path as `quant` (one buffer per mate)
@@ -827,6 +869,10 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   cur_start2_ = 0;
   cur_notag_ = nullptr;
   cur_alt_start_ = cur_alt_start2_ = 0;
+  // the records need the whole batch, and the batch's read-set fields (barcodes, skip and tag marks) are rewritten by
+  // the next one: this path does not overlap batches
+  join();
+  const int32_t* handles = aa_ ? cfc_handles_.p : bws_->slot[last_slot_].d_handles.p;
   launch_bus_records(dd_, handles, n_sets, base, bus_next_id_, bus_idof_.p, bus_isnew_.p, bus_newrank_.p,
                      bus_ismapped_.p, bus_rank_.p, (const uint64_t*)bus_bc_.p, (const uint64_t*)bus_umi_.p, bus_flags_.p,
                      bus_rec_.p, bus_tmp_.p, bus_tmp_.n, st);
@@ -887,8 +933,11 @@ void Quant::set_aa(bool on) {
                   "target in every frame's intersection (dfk_onlist), which makes the result depend on the order of the hits");
     // 6 frames per read set go through the pseudoalignment buffers
     const size_t frames = 6 * (size_t)opt_.max_batch_reads;
-    bws_->d_handles.grow(frames);
-    bws_->d_qentries.grow(frames * KB_Q_STRIDE);
+    for (BatchSlot& w : bws_->slot) {
+      w.d_handles.grow(frames);
+      w.d_qentries.grow(frames * KB_Q_STRIDE);
+      w.d_rlen.grow(frames);
+    }
     cfc_clashes_.grow(1);
     cfc_clashes_.zero(stream_);
   }
@@ -897,6 +946,7 @@ void Quant::set_aa(bool on) {
 
 uint64_t Quant::frame_clashes() {
   unsigned long long c = 0;
+  join();
   if (aa_) {
     cfc_clashes_.download(&c, 1, 0, stream_);
     KB_CK(cudaStreamSynchronize(stream_));
@@ -906,6 +956,7 @@ uint64_t Quant::frame_clashes() {
 
 void Quant::bus_lengths(uint32_t* bc_hist, uint32_t* umi_hist) {
   uint32_t h[66] = {0};
+  join();
   if (bus_hist_.n >= 66) {
     bus_hist_.download(h, 66, 0, stream_);
     KB_CK(cudaStreamSynchronize(stream_));
@@ -959,6 +1010,7 @@ Stats Quant::stats() {
     }
   }
   unsigned long long st[4];
+  sync();
   KB_CK(cudaMemcpy(st, dd_.stats, sizeof(st), cudaMemcpyDeviceToHost));
   s.n_probes = st[0];
   s.n_resolved = st[1];
@@ -1180,6 +1232,7 @@ EmProblem EmWs::problem(uint32_t n_ec, uint32_t T, uint32_t n_multi, int max_ite
 
 EmResult Quant::run_em(const EcTable& ecs, const std::vector<double>& fl_trunc, int max_iter, int min_rounds) {
   KB_CK(cudaSetDevice(ix_.device));
+  join();
   const FlatIndex& f = ix_.flat;
   const uint32_t T = f.num_targets(), nE = ecs.n();
   cudaStream_t st = stream_;
@@ -1228,6 +1281,7 @@ void Quant::set_priors(const double* priors) {
 
 // Used handles, sorted by first occurrence; their lengths and offsets.  First-occurrence keys are distinct per set.
 EcNumbering Quant::number_ecs() {
+  join();
   cudaStream_t st = stream_;
   EmWs& w = *emws_;
   EcNumbering nu;
@@ -1330,6 +1384,7 @@ EmResult Quant::run_em_device(const std::vector<double>& fl_trunc, int max_iter,
 std::vector<int> Quant::run_bootstrap_device(const std::vector<double>& fl_trunc, uint64_t seed, int B, std::vector<double>& alpha_out,
                                              std::vector<uint32_t>* samples_out, double* ms_out) {
   KB_CK(cudaSetDevice(ix_.device));
+  join();
   std::vector<int> rounds;
   if (B <= 0) { alpha_out.clear(); return rounds; }
   if (!dev_problem_valid_) run_em_device(fl_trunc);      // builds the matrices (and runs the main EM once)
@@ -1435,6 +1490,7 @@ void Quant::export_prepare(uint32_t* n_sets, uint32_t* n_entries) {
 
 void Quant::export_copy(uint32_t* d_off, uint32_t* d_tids, uint32_t* d_counts, unsigned long long* d_first) {
   KB_CK(cudaSetDevice(ix_.device));
+  join();
   EmWs& w = *emws_;
   cudaStream_t st = stream_;
   if (exp_n_) {
@@ -1501,6 +1557,7 @@ uint64_t Quant::merge_local(const std::vector<Quant*>& others, uint64_t first_st
 void Quant::import_sets_device(uint32_t n_sets, const uint32_t* d_off, const uint32_t* d_tids, const uint32_t* d_counts,
                                const unsigned long long* d_first, unsigned long long first_offset) {
   KB_CK(cudaSetDevice(ix_.device));
+  join();
   ecs_valid_ = false;
   dev_stats_valid_ = false;
   dev_problem_valid_ = false;

@@ -42,17 +42,25 @@ struct DBuf {
   void zero(cudaStream_t st = 0);
 };
 
+// Everything one batch's kernels write that the next batch's would overwrite.  A run keeps two: batch i uses
+// BatchWs::slot[i & 1] on the run's internal stream i & 1 (Quant::run_batch), so that batch i + 1 can run while batch i
+// drains, and stream order alone keeps batch i + 2 off the buffers until batch i is done with them.
+struct BatchSlot {
+  DBuf<uint32_t> d_counters;        // KB_BATCH_COUNTER_WORDS: the queue counts and match_kernel's hand-out counter
+  DBuf<uint32_t> d_qentries, d_scratch, d_packed, d_rlen;
+  DBuf<uint32_t> d_spill, d_qbig;   // fragments with more than KB_MAX_E distinct EC sets (d_spill: per resident lane)
+  DBuf<int32_t> d_handles;
+  DBuf<uint16_t> d_tl;
+  DBuf<uint8_t> d_skip;             // per fragment: holds a D-list k-mer (only when the index has a D-list)
+};
+
 // Grow-only device work buffers.  They belong to the Index and are lent to one run at a time, so that
 // consecutive runs on the same index (the normal case) do not pay cudaMalloc again; a second run
 // created while the first is still alive gets private ones.
 struct BatchWs {
   DBuf<uint8_t> stage_b[2][2];      // double-buffered input staging: H2D of batch i+1 overlaps the kernels of batch i
   DBuf<uint32_t> stage_o[2][2];
-  DBuf<uint32_t> d_qcount, d_qentries, d_scratch, d_packed;
-  DBuf<uint32_t> d_spill, d_qbig_count, d_qbig;   // fragments with more than KB_MAX_E distinct EC sets
-  DBuf<int32_t> d_handles;
-  DBuf<uint16_t> d_tl;
-  DBuf<uint8_t> d_skip;             // per fragment: holds a D-list k-mer (only when the index has a D-list)
+  BatchSlot slot[2];
 };
 
 // The per-problem device state of launch_em for up to `cap` problems (grow-only), and the one host-side driver of every
@@ -239,10 +247,12 @@ class Quant {
   // cardinality_clashes of the run: frames whose set was as small as the winning frame's before them
   uint64_t frame_clashes();
   // Same, inputs already resident in device memory; handles stay on the device
-  // (device_handles(), valid until the next batch).
+  // (device_handles(), valid until the next batch).  The call returns once the kernels are enqueued; the caller may
+  // overwrite its input in the run's stream order, since that stream waits for the kernels that read it.
   void pseudoalign_device(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
                           uint32_t max_read_len);
-  const int32_t* device_handles() const { return bws_->d_handles.p; }
+  // the last batch's handles, complete in the run's stream order
+  const int32_t* device_handles() { join(); return bws_->slot[last_slot_].d_handles.p; }
   void sync();
 
   // MasterProcessor tail flush + EC id assignment: the table export_prepare lays out on the device (ids from
@@ -313,6 +323,9 @@ class Quant {
   void run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
                  uint32_t max_read_len, const uint8_t* d_bases2 = nullptr, const uint32_t* d_off2 = nullptr);
   void check_device_errors();
+  // Makes the run's stream wait for the batches enqueued on the internal streams since the last join.  Every entry point
+  // that reads or changes run state on the run's stream calls it first.
+  void join();
   // The one EC numbering of every path: the used sets, ids in order of first occurrence, with their handles, counts,
   // lengths and table offsets in emws_.  Synchronises the stream.
   EcNumbering number_ecs();
@@ -323,6 +336,13 @@ class Quant {
   QuantOptions opt_;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = true;
+  // batch i runs on bstream_[i & 1] with BatchWs::slot[i & 1]: forked from stream_ by ev_fork_, stream_ waits for its
+  // input to be read (ev_packed_) and, at the next join(), for all of it (ev_last_)
+  cudaStream_t bstream_[2] = {nullptr, nullptr};
+  cudaEvent_t ev_fork_ = nullptr, ev_packed_[2] = {nullptr, nullptr}, ev_last_[2] = {nullptr, nullptr};
+  uint64_t n_batches_ = 0;
+  int last_slot_ = 0;
+  bool pending_ = false;      // batches enqueued since the last join()
   bool timing_ = false;
   std::vector<cudaEvent_t> events_;   // triples
   Timings tacc_;

@@ -55,6 +55,8 @@ struct BatchArgs {
   uint32_t* qbig_entries;   // stride KB_QBIG_STRIDE
   uint32_t qbig_cap;        // entries
   const uint32_t* packed;   // pack_kernel output: per read, nb 64-bit base words then nb 32-bit invalid masks
+  uint32_t* rlen;           // pack_kernel output: per read, the length read_span gives it (match_kernel reads no input)
+  uint32_t* take;           // match_kernel's hand-out counter: fragments claimed so far (zeroed with the queue counts)
   uint32_t nb;              // 32-base words per packed read = ceil(max_read_len / 32)
   uint32_t pstride;         // 32-bit words per packed read (multiple of 8 = 32 bytes)
   uint32_t empty_ec;        // handle of the empty index EC set, or 0xFFFFFFFF
@@ -76,6 +78,10 @@ struct BatchArgs {
   int no_count;
   uint32_t* first_hit;
 };
+// The counters of one batch, one 128-byte line each (they are zeroed together): q_count at word 0, qbig_count at word
+// KB_BATCH_COUNTER_LINE, match_kernel's hand-out counter `take` at word 2 * KB_BATCH_COUNTER_LINE.
+static constexpr int KB_BATCH_COUNTER_LINE = 32;
+static constexpr int KB_BATCH_COUNTER_WORDS = 3 * KB_BATCH_COUNTER_LINE;
 static constexpr int KB_Q_STRIDE = 2 + KB_MAX_E + 6;   // frag, n|flags, handles, 2 strand words, 4 position-filter words
 static constexpr int KB_SPILL = 112;                   // a fragment may hit KB_MAX_E + KB_SPILL = 128 distinct EC sets
 static constexpr int KB_QBIG_STRIDE = 2 + KB_MAX_E + KB_SPILL + 6;
@@ -102,9 +108,11 @@ void launch_dict_init(const DictInitArgs& a, cudaStream_t st);
 
 // Pseudoalignment of one batch: match kernel (thread per fragment) + resolve kernel (warp per
 // queued fragment) [+ fragment-length finalisation].
-// ev (optional): three events recorded before match_kernel, between the kernels, after resolve_kernel.
+// ev (optional): four events recorded before pack_kernel, before match_kernel, between the kernels, after
+// resolve_kernel.  packed (optional): recorded once the kernels that read the batch's input (bases, offsets) are done;
+// the later kernels read only what they wrote to ba's work buffers.
 void launch_pseudoalign(const DevIndex& ix, const DevDict& dd, const BatchArgs& ba, const ResolveArgs& ra,
-                        int threads_per_block, cudaStream_t st, cudaEvent_t* ev = nullptr);
+                        int threads_per_block, cudaStream_t st, cudaEvent_t* ev = nullptr, cudaEvent_t packed = nullptr);
 void launch_fld_finalize(const DevDict& dd, const BatchArgs& ba, cudaStream_t st);
 void launch_import_sets(const DevDict& dd, uint32_t n_sets, const uint32_t* off, const uint32_t* tids, const uint32_t* counts,
                         const unsigned long long* first, unsigned long long first_offset, cudaStream_t st);

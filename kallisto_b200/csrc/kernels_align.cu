@@ -224,6 +224,7 @@ __global__ void __launch_bounds__(256) pack_kernel(BatchArgs ba, uint32_t n_read
   int len;
   const uint8_t* src_bases;
   read_span(ba, r, src_bases, off, len);
+  if (w == 0) ba.rlen[r] = (uint32_t)len;
   const int base = (int)w * 32;
   uint32_t hi = 0, lo = 0, inv32 = ~0u;
   if (base < len) {
@@ -369,12 +370,10 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
                 "a tuple grown by 6 words past KB_MAX_E overwrites exactly the first-hit words of both chains");
   auto cw = [&](int w, int c) -> uint32_t& { return cold[(size_t)(2 * w + c) * nt]; };
 
-  // contiguous chunk of fragments owned by this warp
-  const uint32_t n_warps = (gridDim.x * nt) >> 5;
-  const uint32_t gw = (blockIdx.x * nt + tid) >> 5;
-  const uint32_t chunk = (ba.n_frag + n_warps - 1) / n_warps;
-  uint32_t next = min(ba.n_frag, gw * chunk);
-  const uint32_t end = min(ba.n_frag, next + chunk);
+  // fragments are handed out at each refill from one counter for the whole grid, as many as the warp has idle lanes: a
+  // warp whose fragments were quick takes more, so the warps run out of work together instead of each draining a
+  // fixed share (and the blocks of a launch that become resident late take only what is left)
+  bool work_left = true;     // warp-uniform: the counter has not passed n_frag yet
   const int n_mates = ba.paired ? 2 : 1;
   const int n_chunks = (int)(ba.pstride >> 3);   // 32-byte pieces per packed read
 
@@ -436,7 +435,6 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
     const bool done = st[0] == S_FIN && st[1] == S_FIN;
     const unsigned fin = __ballot_sync(0xFFFFFFFFu, done);
     const unsigned idle = fin | __ballot_sync(0xFFFFFFFFu, st[0] == S_EMPTY);
-    const bool work_left = next < end;
     if (idle == 0xFFFFFFFFu && fin == 0 && !work_left) break;
     KB_MS_ONLY(in_service = false;)
     if (idle == 0xFFFFFFFFu || (work_left && __popc(idle) >= ba.refill_min)) {
@@ -583,24 +581,27 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
         st[0] = st[1] = S_EMPTY;
       }
       __syncwarp();
-      // ---- refill: the idle lanes take the next fragments of the warp's chunk and copy their packed
-      //      reads (pack_kernel output) into shared memory with 32-byte loads (ld256_nc)
-      {
+      // ---- refill: the idle lanes claim the next fragments with one atomic of lane 0 and copy their packed reads
+      //      (pack_kernel output) into shared memory with 32-byte loads (ld256_nc)
+      if (work_left) {
+        const uint32_t n_idle = __popc(idle);
+        uint32_t f0 = 0;
+        if (lane == 0) f0 = atomicAdd(ba.take, n_idle);
+        f0 = __shfl_sync(0xFFFFFFFFu, f0, 0);
+        const uint32_t avail = f0 < ba.n_frag ? ba.n_frag - f0 : 0u;
+        if (avail <= n_idle) work_left = false;
         const bool is_idle = (idle >> lane) & 1u;
         const uint32_t rank = __popc(idle & ((1u << lane) - 1));
-        const uint32_t avail = end - next;
         if (is_idle && rank < avail) {
-          const uint32_t fidx = next + rank;
+          const uint32_t fidx = f0 + rank;
           unsigned inv = 0;
 #pragma unroll
           for (int mt = 0; mt < 2; ++mt) {
             len[mt] = 0;
             if (mt >= n_mates) continue;
             const uint32_t ridx = ba.paired ? 2 * fidx + mt : fidx;
-            const uint8_t* unused_base;
-            uint64_t unused_off;
-            int l;
-            read_span(ba, ridx, unused_base, unused_off, l);
+            // read_span's length, as pack_kernel found it; the D-list marks come after packing
+            int l = (ba.skip && ba.skip[fidx]) ? 0 : (int)ba.rlen[ridx];
             if (l > nb * 32) l = nb * 32;   // cannot happen: the host sizes nb from the longest read
             len[mt] = l;
             const uint32_t* src = ba.packed + (size_t)ridx * ba.pstride;
@@ -640,8 +641,6 @@ __global__ void __launch_bounds__(256, KB_MATCH_MIN_BLOCKS) match_kernel(DevInde
             }
           }
         }
-        const uint32_t n_idle = __popc(idle);
-        next += n_idle < avail ? n_idle : avail;
       }
       continue;
     }
@@ -1111,10 +1110,9 @@ __global__ void collect_used_kernel(DevDict dd, uint32_t* used, uint32_t* n_used
 }
 
 void launch_pseudoalign(const DevIndex& ix, const DevDict& dd, const BatchArgs& ba, const ResolveArgs& ra,
-                        int tpb, cudaStream_t st, cudaEvent_t* ev) {
+                        int tpb, cudaStream_t st, cudaEvent_t* ev, cudaEvent_t packed) {
   if (ba.n_frag == 0) return;
-  cudaMemsetAsync(ba.q_count, 0, sizeof(uint32_t), st);
-  cudaMemsetAsync(ba.qbig_count, 0, sizeof(uint32_t), st);
+  cudaMemsetAsync(ba.q_count, 0, sizeof(uint32_t) * KB_BATCH_COUNTER_WORDS, st);   // q_count, qbig_count, take
   // persistent grid: as many blocks as fit on the device at once
   const size_t smem = (size_t)tpb * 4 * match_lane_words(ba.nb);
   const int sms = device_sm_count();
@@ -1132,6 +1130,7 @@ void launch_pseudoalign(const DevIndex& ix, const DevDict& dd, const BatchArgs& 
     pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ba, n_reads, const_cast<uint32_t*>(ba.packed));
     if (ix.dfk && ba.skip_w) dlist_scan_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ix, ba, n_reads);
   }
+  if (packed) cudaEventRecord(packed, st);    // the batch's input buffers are not read after this point
   if (ev) cudaEventRecord(ev[1], st);
 #ifdef KB_MATCH_STATS
   void* ms_dev = nullptr;
