@@ -526,8 +526,7 @@ void Quant::check_device_errors() {
   throw Error(m);
 }
 
-void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
-                      uint32_t max_read_len, const uint8_t* d_bases2, const uint32_t* d_off2) {
+void Quant::run_batch(BatchArgs ba, uint32_t n_reads, uint32_t max_read_len) {
   const uint32_t n_frag = opt_.paired ? n_reads / 2 : n_reads;
   if (opt_.paired && (n_reads & 1)) throw Error("kallisto_b200: odd number of reads in a paired batch");
   const int b = (int)(n_batches_ & 1);
@@ -545,12 +544,6 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ecs_valid_ = false;
   dev_stats_valid_ = false;
   dev_problem_valid_ = false;
-  BatchArgs ba{};
-  ba.bases = d_bases;
-  ba.off = d_off;
-  ba.bases2 = d_bases2;
-  ba.off2 = d_off2;
-  ba.fixed_len = fixed_len;
   ba.n_frag = n_frag;
   ba.paired = opt_.paired;
   ba.strand_mode = aa_ ? 0 : opt_.strand_mode;     // --aa: the frames are matched unstranded, cfc_select_kernel filters the set
@@ -579,12 +572,11 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
   ba.rlen = w.d_rlen.p;
   ba.empty_ec = ix_.empty_ec;
   ba.refill_min = opt_.refill_min;
-  ba.skip = cur_skip_;
   ba.skip_w = nullptr;
   if (ix_.dev.dfk) {
     // D-list: fragments holding a distinguishing flanking k-mer are marked by dlist_scan_kernel (after packing)
-    if (cur_skip_) {
-      ba.skip_w = const_cast<uint8_t*>(cur_skip_);          // bus: the scan adds to the bad-barcode marks
+    if (ba.skip) {
+      ba.skip_w = const_cast<uint8_t*>(ba.skip);            // bus: the scan adds to the bad-barcode marks
     } else {
       if (w.d_skip.n < n_frag) w.d_skip.alloc(std::max<size_t>(n_frag, opt_.max_batch_reads));
       KB_CK(cudaMemsetAsync(w.d_skip.p, 0, n_frag, bs));
@@ -592,11 +584,6 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
     }
   }
   ba.fp_fl = opt_.fp_fl;
-  ba.start = cur_start_;
-  ba.start2 = cur_start2_;
-  ba.notag = cur_notag_;
-  ba.alt_start = cur_alt_start_;
-  ba.alt_start2 = cur_alt_start2_;
   ba.no_count = aa_ ? 1 : 0;
   ba.first_hit = aa_ ? cfc_first_.p : nullptr;
   ResolveArgs ra{};
@@ -648,48 +635,72 @@ void Quant::run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_
 void Quant::pseudoalign_device(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
                                uint32_t max_read_len) {
   KB_CK(cudaSetDevice(ix_.device));
-  run_batch(d_bases, d_off, n_reads, fixed_len, max_read_len);
+  BatchArgs in{};
+  in.bases = d_bases;
+  in.off = d_off;
+  in.fixed_len = fixed_len;
+  run_batch(in, n_reads, max_read_len);
+}
+
+Quant::Staged Quant::stage(int s, int nf, const char* const* bases, const uint32_t* const* offs, uint32_t n,
+                           uint32_t fixed_len, uint64_t min_bases, size_t min_offs) {
+  Staged g{};
+  KB_CK(cudaStreamWaitEvent(copy_stream_, ev_done_[s], 0));      // kernels that last read this slot
+  for (int k = 0; k < nf; ++k) {
+    const uint32_t* off = offs[k];
+    const uint64_t n_bases = off ? off[n] : (uint64_t)n * fixed_len;
+    DBuf<uint8_t>& db = bws_->stage_b[s][k];
+    if (db.n < n_bases + 16) { KB_CK(cudaStreamSynchronize(stream_)); db.alloc(std::max<uint64_t>(n_bases + 16, min_bases)); }
+    KB_CK(cudaMemcpyAsync(db.p, bases[k], n_bases, cudaMemcpyHostToDevice, copy_stream_));
+    g.bases[k] = db.p;
+    g.maxlen[k] = fixed_len;
+    if (off) {
+      DBuf<uint32_t>& dofs = bws_->stage_o[s][k];
+      if (dofs.n < (size_t)n + 1) { KB_CK(cudaStreamSynchronize(stream_)); dofs.alloc(std::max<size_t>((size_t)n + 1, min_offs)); }
+      KB_CK(cudaMemcpyAsync(dofs.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, copy_stream_));
+      g.off[k] = dofs.p;
+      g.maxlen[k] = 0;
+      for (uint32_t i = 0; i < n; ++i) g.maxlen[k] = std::max(g.maxlen[k], off[i + 1] - off[i]);
+    }
+  }
+  KB_CK(cudaEventRecord(ev_copied_[s], copy_stream_));
+  KB_CK(cudaStreamWaitEvent(stream_, ev_copied_[s], 0));
+  return g;
+}
+
+void Quant::pseudoalign_staged(int nf, const char* const* bases, const uint32_t* const* offs, uint32_t n,
+                               uint32_t fixed_len, int32_t* handles_out) {
+  // batches alternate between the two staging slots, so that the copy of one overlaps the previous batch's kernels
+  const int s = stage_idx_;
+  stage_idx_ ^= 1;
+  // first allocations: one buffer holds a whole batch, a mate's buffer half of it
+  const Staged g = nf == 1 ? stage(s, 1, bases, offs, n, fixed_len, opt_.max_batch_bases, 2 * (size_t)opt_.max_batch_reads + 1)
+                           : stage(s, 2, bases, offs, n, fixed_len, opt_.max_batch_bases / 2 + 16, (size_t)opt_.max_batch_reads + 1);
+  BatchArgs in{};
+  in.bases = g.bases[0];
+  in.off = g.off[0];
+  in.bases2 = g.bases[1];
+  in.off2 = g.off[1];
+  in.fixed_len = fixed_len;
+  const uint32_t n_reads = (uint32_t)nf * n;
+  run_batch(in, n_reads, std::max(g.maxlen[0], g.maxlen[1]));
+  KB_CK(cudaEventRecord(ev_done_[s], stream_));
+  if (handles_out) {
+    join();
+    bws_->slot[last_slot_].d_handles.download(handles_out, opt_.paired ? n_reads / 2 : n_reads, 0, stream_);
+    KB_CK(cudaStreamSynchronize(stream_));
+  } else {
+    // the caller may reuse its buffers once the copy is done; the kernels keep running
+    KB_CK(cudaEventSynchronize(ev_copied_[s]));
+  }
 }
 
 void Quant::pseudoalign_host(const char* bases, const uint32_t* off, uint32_t n_reads, uint32_t fixed_len,
                              int32_t* handles_out) {
   KB_CK(cudaSetDevice(ix_.device));
   if (n_reads == 0) return;
-  uint64_t n_bases;
-  uint32_t maxlen = fixed_len;
-  if (off) {
-    n_bases = off[n_reads];
-    maxlen = 0;
-    for (uint32_t i = 0; i < n_reads; ++i) maxlen = std::max(maxlen, off[i + 1] - off[i]);
-    if (off[0] != 0) throw Error("kallisto_b200: offsets must start at 0");
-  } else {
-    n_bases = (uint64_t)n_reads * fixed_len;
-  }
-  // stage into buffer `s`; the copy runs on its own stream so that it overlaps the previous batch's kernels
-  const int s = stage_idx_;
-  stage_idx_ ^= 1;
-  DBuf<uint8_t>& db = bws_->stage_b[s][0];
-  DBuf<uint32_t>& dofs = bws_->stage_o[s][0];
-  KB_CK(cudaStreamWaitEvent(copy_stream_, ev_done_[s], 0));      // kernels that last read this buffer
-  if (db.n < n_bases + 16) { KB_CK(cudaStreamSynchronize(stream_)); db.alloc(std::max<uint64_t>(n_bases + 16, opt_.max_batch_bases)); }
-  KB_CK(cudaMemcpyAsync(db.p, bases, n_bases, cudaMemcpyHostToDevice, copy_stream_));
-  if (off) {
-    if (dofs.n < (size_t)n_reads + 1) { KB_CK(cudaStreamSynchronize(stream_)); dofs.alloc(std::max<size_t>((size_t)n_reads + 1, (size_t)opt_.max_batch_reads * 2 + 1)); }
-    KB_CK(cudaMemcpyAsync(dofs.p, off, ((size_t)n_reads + 1) * 4, cudaMemcpyHostToDevice, copy_stream_));
-  }
-  KB_CK(cudaEventRecord(ev_copied_[s], copy_stream_));
-  KB_CK(cudaStreamWaitEvent(stream_, ev_copied_[s], 0));
-  run_batch(db.p, off ? dofs.p : nullptr, n_reads, fixed_len, maxlen);
-  KB_CK(cudaEventRecord(ev_done_[s], stream_));
-  if (handles_out) {
-    const uint32_t n_frag = opt_.paired ? n_reads / 2 : n_reads;
-    join();
-    bws_->slot[last_slot_].d_handles.download(handles_out, n_frag, 0, stream_);
-    KB_CK(cudaStreamSynchronize(stream_));
-  } else {
-    // the caller may reuse its buffers once the copy is done; the kernels keep running
-    KB_CK(cudaEventSynchronize(ev_copied_[s]));
-  }
+  if (off && off[0] != 0) throw Error("kallisto_b200: offsets must start at 0");
+  pseudoalign_staged(1, &bases, &off, n_reads, fixed_len, handles_out);
 }
 
 void Quant::pseudoalign_host_pe(const char* bases1, const uint32_t* off1, const char* bases2, const uint32_t* off2,
@@ -698,45 +709,9 @@ void Quant::pseudoalign_host_pe(const char* bases1, const uint32_t* off1, const 
   if (n_pairs == 0) return;
   if (!opt_.paired) throw Error("kallisto_b200: per-mate buffers need a paired run");
   if ((off1 == nullptr) != (off2 == nullptr)) throw Error("kallisto_b200: give offsets for both mates or for neither");
-  uint64_t nb1, nb2;
-  uint32_t maxlen = fixed_len;
-  if (off1) {
-    nb1 = off1[n_pairs];
-    nb2 = off2[n_pairs];
-    maxlen = 0;
-    for (uint32_t i = 0; i < n_pairs; ++i) maxlen = std::max(maxlen, std::max(off1[i + 1] - off1[i], off2[i + 1] - off2[i]));
-  } else {
-    nb1 = nb2 = (uint64_t)n_pairs * fixed_len;
-  }
-  const int s = stage_idx_;
-  stage_idx_ ^= 1;
-  DBuf<uint8_t>& b1 = bws_->stage_b[s][0];
-  DBuf<uint8_t>& b2 = bws_->stage_b[s][1];
-  DBuf<uint32_t>& o1 = bws_->stage_o[s][0];
-  DBuf<uint32_t>& o2 = bws_->stage_o[s][1];
-  KB_CK(cudaStreamWaitEvent(copy_stream_, ev_done_[s], 0));
-  if (b1.n < nb1 + 16) { KB_CK(cudaStreamSynchronize(stream_)); b1.alloc(std::max<uint64_t>(nb1 + 16, opt_.max_batch_bases / 2 + 16)); }
-  if (b2.n < nb2 + 16) { KB_CK(cudaStreamSynchronize(stream_)); b2.alloc(std::max<uint64_t>(nb2 + 16, opt_.max_batch_bases / 2 + 16)); }
-  KB_CK(cudaMemcpyAsync(b1.p, bases1, nb1, cudaMemcpyHostToDevice, copy_stream_));
-  KB_CK(cudaMemcpyAsync(b2.p, bases2, nb2, cudaMemcpyHostToDevice, copy_stream_));
-  if (off1) {
-    const size_t no = (size_t)n_pairs + 1;
-    if (o1.n < no) { KB_CK(cudaStreamSynchronize(stream_)); o1.alloc(std::max<size_t>(no, (size_t)opt_.max_batch_reads + 1)); }
-    if (o2.n < no) { KB_CK(cudaStreamSynchronize(stream_)); o2.alloc(std::max<size_t>(no, (size_t)opt_.max_batch_reads + 1)); }
-    KB_CK(cudaMemcpyAsync(o1.p, off1, no * 4, cudaMemcpyHostToDevice, copy_stream_));
-    KB_CK(cudaMemcpyAsync(o2.p, off2, no * 4, cudaMemcpyHostToDevice, copy_stream_));
-  }
-  KB_CK(cudaEventRecord(ev_copied_[s], copy_stream_));
-  KB_CK(cudaStreamWaitEvent(stream_, ev_copied_[s], 0));
-  run_batch(b1.p, off1 ? o1.p : nullptr, 2 * n_pairs, fixed_len, maxlen, b2.p, off1 ? o2.p : nullptr);
-  KB_CK(cudaEventRecord(ev_done_[s], stream_));
-  if (handles_out) {
-    join();
-    bws_->slot[last_slot_].d_handles.download(handles_out, n_pairs, 0, stream_);
-    KB_CK(cudaStreamSynchronize(stream_));
-  } else {
-    KB_CK(cudaEventSynchronize(ev_copied_[s]));
-  }
+  const char* bases[2] = {bases1, bases2};
+  const uint32_t* offs[2] = {off1, off2};
+  pseudoalign_staged(2, bases, offs, n_pairs, fixed_len, handles_out);
 }
 
 void Quant::bus_batch_host(const char* const* bases, const uint32_t* const* offs, uint32_t n_sets, BusRecord* records_out,
@@ -746,31 +721,18 @@ void Quant::bus_batch_host(const char* const* bases, const uint32_t* const* offs
   if (n_records_out) *n_records_out = 0;
   if (n_sets == 0) return;
   const BusSpec& sp = opt_.bus_spec;
-  cudaStream_t st = stream_;
-  const uint8_t* db[4] = {nullptr, nullptr, nullptr, nullptr};
-  const uint32_t* dofs[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (int k = 0; k < sp.nfiles; ++k) {
+  for (int k = 0; k < sp.nfiles; ++k)
     if (!bases[k] || !offs[k]) throw Error("kallisto_b200: bus batch needs bases and offsets for every file of the technology");
-    const uint64_t nbz = offs[k][n_sets];
-    if (bus_b_[k].n < nbz + 16) bus_b_[k].alloc(std::max<uint64_t>(nbz + 16, opt_.max_batch_bases / 2 + 16));
-    if (bus_o_[k].n < (size_t)n_sets + 1) bus_o_[k].alloc(std::max<size_t>((size_t)n_sets + 1, (size_t)opt_.max_batch_reads + 1));
-    KB_CK(cudaMemcpyAsync(bus_b_[k].p, bases[k], nbz, cudaMemcpyHostToDevice, st));
-    KB_CK(cudaMemcpyAsync(bus_o_[k].p, offs[k], ((size_t)n_sets + 1) * 4, cudaMemcpyHostToDevice, st));
-    db[k] = bus_b_[k].p;
-    dofs[k] = bus_o_[k].p;
-  }
+  // This path does not overlap batches, so it stages into slot 0 only, once the run's stream is done with the batch
+  // before: bus_fields, cfc_frames and pack_kernel all read the staged files, and that batch may have failed part way.
+  KB_CK(cudaEventRecord(ev_done_[0], stream_));
+  const Staged g = stage(0, sp.nfiles, bases, offs, n_sets, 0, opt_.max_batch_bases / 2 + 16, (size_t)opt_.max_batch_reads + 1);
   // longest cDNA read of the batch (sizes the packed-read layout)
-  uint32_t maxlen = 0;
-  const uint32_t* so = offs[sp.seq_file];
-  for (uint32_t i = 0; i < n_sets; ++i) maxlen = std::max(maxlen, so[i + 1] - so[i]);
-  if (sp.paired) {
-    so = offs[sp.seq2_file];
-    for (uint32_t i = 0; i < n_sets; ++i) maxlen = std::max(maxlen, so[i + 1] - so[i]);
-  }
-  const uint32_t n_rec = bus_core(db, dofs, n_sets, maxlen);
+  const uint32_t maxlen = std::max(g.maxlen[sp.seq_file], sp.paired ? g.maxlen[sp.seq2_file] : 0u);
+  const uint32_t n_rec = bus_core(g.bases, g.off, n_sets, maxlen);
   if (n_rec && records_out) {
-    bus_rec_.download(records_out, n_rec, 0, st);
-    KB_CK(cudaStreamSynchronize(st));
+    bus_rec_.download(records_out, n_rec, 0, stream_);
+    KB_CK(cudaStreamSynchronize(stream_));
   }
   if (n_records_out) *n_records_out = n_rec;
 }
@@ -812,20 +774,23 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   launch_bus_fields(a, st);
   KB_CK(cudaGetLastError());
   // the cDNA read(s): single-read or paired pseudoalignment with the strand filter of the technology
+  BatchArgs in{};
+  in.bases = db[sp.seq_file];
+  in.off = dofs[sp.seq_file];
+  in.start = (uint32_t)sp.seq_start;
+  in.skip = bus_skip_.p;
   uint32_t min_start = (uint32_t)(sp.paired ? std::min(sp.seq_start, sp.seq2_start) : sp.seq_start);
   if (sp.tag_len) {
     // a read set without the tag has no UMI: the sequence read that shares the UMI's file starts where the tag would
     // have started (src/ProcessReads.cpp:1547,1553-1554), the other one where the technology says
     const int at = sp.umi_a[0] - sp.tag_len;
-    cur_notag_ = bus_notag_.p;
-    cur_alt_start_ = (uint32_t)(sp.umi_f[0] == sp.seq_file ? at : sp.seq_start);
-    cur_alt_start2_ = (uint32_t)(sp.paired && sp.umi_f[0] == sp.seq2_file ? at : sp.seq2_start);
-    min_start = std::min(min_start, sp.paired ? std::min(cur_alt_start_, cur_alt_start2_) : cur_alt_start_);
+    in.notag = bus_notag_.p;
+    in.alt_start = (uint32_t)(sp.umi_f[0] == sp.seq_file ? at : sp.seq_start);
+    in.alt_start2 = (uint32_t)(sp.paired && sp.umi_f[0] == sp.seq2_file ? at : sp.seq2_start);
+    min_start = std::min(min_start, sp.paired ? std::min(in.alt_start, in.alt_start2) : in.alt_start);
   }
   maxlen = maxlen > min_start ? maxlen - min_start : 1;
   const uint64_t base = n_frag_total_;
-  cur_skip_ = bus_skip_.p;
-  cur_start_ = (uint32_t)sp.seq_start;
   if (aa_) {
     // the six reading frames of every set in comma-free code (kernels_cfc.cu), 6 n_sets unpaired fragments; a skipped
     // set has empty frames
@@ -853,22 +818,20 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
     launch_cfc_frames(c, st);
     KB_CK(cudaGetLastError());
     n_kernel_launches += 2;      // cfc_len, cfc_frames
-    cur_skip_ = nullptr;
-    cur_start_ = 0;
-    run_batch(cfc_b_.p, cfc_o_.p, 6 * n_sets, 0, maxlen);
+    BatchArgs fr{};              // the frames, from their first base and without skip marks: a skipped set's are empty
+    fr.bases = cfc_b_.p;
+    fr.off = cfc_o_.p;
+    run_batch(fr, 6 * n_sets, maxlen);
   } else if (sp.paired) {
     // two sequence reads (busopt.paired, src/ProcessReads.cpp:1550-1567,1646-1650): the pair goes through the same
     // match x 2 / intersectKmers / strand filter / mapPair path as `quant` (one buffer per mate)
-    cur_start2_ = (uint32_t)sp.seq2_start;
-    run_batch(db[sp.seq_file], dofs[sp.seq_file], 2 * n_sets, 0, maxlen, db[sp.seq2_file], dofs[sp.seq2_file]);
+    in.bases2 = db[sp.seq2_file];
+    in.off2 = dofs[sp.seq2_file];
+    in.start2 = (uint32_t)sp.seq2_start;
+    run_batch(in, 2 * n_sets, maxlen);
   } else {
-    run_batch(db[sp.seq_file], dofs[sp.seq_file], n_sets, 0, maxlen);
+    run_batch(in, n_sets, maxlen);
   }
-  cur_skip_ = nullptr;
-  cur_start_ = 0;
-  cur_start2_ = 0;
-  cur_notag_ = nullptr;
-  cur_alt_start_ = cur_alt_start2_ = 0;
   // the records need the whole batch, and the batch's read-set fields (barcodes, skip and tag marks) are rewritten by
   // the next one: this path does not overlap batches
   join();

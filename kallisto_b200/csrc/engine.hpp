@@ -58,8 +58,10 @@ struct BatchSlot {
 // consecutive runs on the same index (the normal case) do not pay cudaMalloc again; a second run
 // created while the first is still alive gets private ones.
 struct BatchWs {
-  DBuf<uint8_t> stage_b[2][2];      // double-buffered input staging: H2D of batch i+1 overlaps the kernels of batch i
-  DBuf<uint32_t> stage_o[2][2];
+  // input staging of the host entry points (Quant::stage), up to four files per slot: the quant runs alternate between
+  // the slots, so that the copy of batch i+1 overlaps the kernels of batch i; the bus runs use slot 0
+  DBuf<uint8_t> stage_b[2][4];
+  DBuf<uint32_t> stage_o[2][4];
   BatchSlot slot[2];
 };
 
@@ -320,8 +322,24 @@ class Quant {
   uint64_t dev_n_ecs_ = 0, dev_nnz_ = 0, dev_pseudoaligned_ = 0, dev_unique_ = 0;
 
  private:
-  void run_batch(const uint8_t* d_bases, const uint32_t* d_off, uint32_t n_reads, uint32_t fixed_len,
-                 uint32_t max_read_len, const uint8_t* d_bases2 = nullptr, const uint32_t* d_off2 = nullptr);
+  // `in`: the batch's input and layout, the fields of BatchArgs its caller fills (kernels.hpp); run_batch fills the rest
+  void run_batch(BatchArgs in, uint32_t n_reads, uint32_t max_read_len);
+  // A host batch on the device: per file, its bases, its offsets (nullptr without) and its longest read.
+  struct Staged {
+    const uint8_t* bases[4];
+    const uint32_t* off[4];
+    uint32_t maxlen[4];
+  };
+  // The one host-to-device copy of reads: the files k < nf of a batch of n reads each (bases [0, offs[k][n]), or
+  // n x fixed_len without offsets, since offsets are positions in bases[k] and need not start at 0) into staging slot s
+  // on copy_stream_, after the kernels that last read the slot (ev_done_[s]); the run's stream waits for the copy
+  // (ev_copied_[s]).  A buffer that is too small is reallocated to at least min_bases / min_offs.
+  Staged stage(int s, int nf, const char* const* bases, const uint32_t* const* offs, uint32_t n, uint32_t fixed_len,
+               uint64_t min_bases, size_t min_offs);
+  // pseudoalign_host (nf = 1: one buffer of n reads) and pseudoalign_host_pe (nf = 2: one buffer of n reads per mate)
+  // after their checks
+  void pseudoalign_staged(int nf, const char* const* bases, const uint32_t* const* offs, uint32_t n, uint32_t fixed_len,
+                          int32_t* handles_out);
   void check_device_errors();
   // Makes the run's stream wait for the batches enqueued on the internal streams since the last join.  Every entry point
   // that reads or changes run state on the run's stream calls it first.
@@ -376,8 +394,8 @@ class Quant {
   bool has_priors_ = false;
   struct EmWs* emws_ = nullptr;
   // bus mode
-  DBuf<uint8_t> bus_b_[4], bus_skip_, bus_notag_;
-  DBuf<uint32_t> bus_o_[4], bus_flags_, bus_hist_, bus_isnew_, bus_newrank_, bus_ismapped_, bus_rank_;
+  DBuf<uint8_t> bus_skip_, bus_notag_;
+  DBuf<uint32_t> bus_flags_, bus_hist_, bus_isnew_, bus_newrank_, bus_ismapped_, bus_rank_;
   DBuf<unsigned long long> bus_bc_, bus_umi_, bus_nvalid_;
   DBuf<int32_t> bus_idof_;
   DBuf<BusRecord> bus_rec_;
@@ -387,9 +405,6 @@ class Quant {
   DBuf<unsigned long long> lm_first_;
   uint32_t bus_next_id_ = 0;
   uint64_t bus_valid_total_ = 0, bus_sample_base_ = 0;
-  const uint8_t* cur_skip_ = nullptr;
-  uint32_t cur_start_ = 0, cur_start2_ = 0, cur_alt_start_ = 0, cur_alt_start2_ = 0;
-  const uint8_t* cur_notag_ = nullptr;
   // bus --aa: the frames of a batch (6 per read set), frame 0's first hit per set, the sets' handles, the clash count
   bool aa_ = false;
   DBuf<uint8_t> cfc_b_, cfc_tmp_;

@@ -36,6 +36,8 @@ struct DictInitArgs {
 
 // One batch of reads for the pseudoalignment kernels (ReadProcessor::processBuffer's `seqs`,
 // src/ProcessReads.cpp:968-1046): concatenated ASCII bases, mates interleaved when paired.
+// The caller of Quant::run_batch fills the batch's input and its layout: bases, off, bases2, off2, fixed_len, start,
+// start2, skip, notag, alt_start and alt_start2 (zero or nullptr when not in play).  run_batch fills in the rest.
 struct BatchArgs {
   const uint8_t* bases;
   const uint32_t* off;      // n_reads + 1 offsets into bases, or nullptr when every read has fixed_len bases
