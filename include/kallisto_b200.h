@@ -325,6 +325,42 @@ int kb_bus_set_aa(kb_quant* q, int32_t on);
  * is as small as the smallest one before them. */
 int kb_bus_frame_clashes(kb_quant* q, uint64_t* n_out);
 
+/* ---- `kallisto bus --devices`: batches of one read stream dealt to several bus runs (one index replica each, on one GPU
+ * or several), with the records and the EC table a single run fed the whole stream would produce.  Every batch is
+ * numbered run-wide on its member (first-occurrence keys, --num read numbers); when a batch completes, the sets that
+ * were new on its member are committed in order of first occurrence to the group's registry (transcript list -> id): a
+ * set the registry knows keeps its id, an unknown one takes the next.  One host thread drives a group; it is not
+ * thread-safe.  Refusals return KB_ERR_INVALID. */
+typedef struct kb_bus_group kb_bus_group;
+/* members: n >= 1 fresh kb_bus_create handles (no batch run yet, none listed twice), with identical kb_bus_opts, --aa and
+ * batch-barcode settings, on indices with the same k and target count.  The same device may appear more than once.  The
+ * group does not own the members: free it before them. */
+int kb_bus_group_create(kb_quant* const* members, int32_t n, kb_bus_group** out);
+void kb_bus_group_free(kb_bus_group* g);
+/* Stages one batch (as kb_bus_batch) on `member` and enqueues its work; returns once the host buffers may be reused.
+ * *ticket numbers the batches of the group in submission order.  A member takes one batch at a time: a member with a
+ * batch outstanding is refused. */
+int kb_bus_group_submit(kb_bus_group* g, int32_t member, const char* const* bases, const uint32_t* const* offsets,
+                        uint32_t n_sets, uint64_t* ticket);
+/* Finishes the oldest outstanding batch, whose ticket must be given (any other is refused): records_out (capacity: its
+ * n_sets) receives its records, in read order, with run-wide EC ids.  A batch kb_bus_batch would fail (--batch-barcodes
+ * with a barcode over 32 letters) fails here. */
+int kb_bus_group_complete(kb_bus_group* g, uint64_t ticket, kb_bus_record* records_out, uint32_t* n_records_out);
+/* kb_bus_begin_sample on every member, and --num read numbers restart run-wide.  Refused while a batch is outstanding. */
+int kb_bus_group_begin_sample(kb_bus_group* g, uint64_t barcode);
+/* n_processed, n_pseudoaligned, n_unique and the lookup counters summed over the members; n_ecs / n_ec_entries of the
+ * group's numbering. */
+int kb_bus_group_finalize(kb_bus_group* g, kb_run_stats* stats);
+/* The group's EC table (layout of kb_quant_ec_table, ids in run-wide order), counts summed over the members. */
+int kb_bus_group_ec_table(kb_bus_group* g, uint64_t* ec_offsets /* n_ecs+1 */, uint32_t* tids /* n_ec_entries */,
+                          uint32_t* counts /* n_ecs */);
+/* Barcode / UMI length histograms summed over the members (kb_bus_lengths). */
+int kb_bus_group_lengths(kb_bus_group* g, uint32_t* bc_hist, uint32_t* umi_hist);
+/* --aa: frame clashes summed over the members (kb_bus_frame_clashes). */
+int kb_bus_group_frame_clashes(kb_bus_group* g, uint64_t* n_out);
+/* Fragment lengths are those of member 0 (kb_quant_get_flens on it): a driver that wants the first 10000 pairs of each
+ * sample gives member 0 the sample's batches until its histogram holds 10000. */
+
 /* Host-only: parse a FASTA/FASTQ file (plain or gzip) with the library's reader (kseq_read grammar,
  * src/kseq.h) and report the number of records, of bases, and an FNV-1a hash of the sequences
  * (0xFF after each record).  Tooling / tests. */

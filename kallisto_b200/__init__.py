@@ -18,6 +18,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KB_LIB_PATH") or os.path.join(_HERE, "libkallisto_b200.so")   # KB_LIB_PATH: experiments only
 
 KB_OK = 0
+KB_ERR_INVALID = -1
 KB_ERR_NO_DEVICE = -3
 
 
@@ -100,7 +101,7 @@ EXPORTED_SYMBOLS = [
     "kb_quant_get_timings", "kb_quant_finalize", "kb_quant_ec_table", "kb_quant_get_flens",
     "kb_quant_set_flens", "kb_em_run", "kb_em_run_table", "kb_read_priors", "kb_em_set_priors", "kb_bootstrap_run", "kb_quant_export_prepare", "kb_quant_export_device", "kb_quant_import_device",
     "kb_comm_unique_id", "kb_comm_create", "kb_comm_create_from_nccl", "kb_comm_create_all", "kb_comm_reserve", "kb_comm_free",
-    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_run_priors", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_set_batch_barcodes", "kb_bus_lengths", "kb_bus_set_aa", "kb_bus_frame_clashes", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
+    "kb_quant_merge_nccl", "kb_quant_merge_local", "kb_quant_set_frag_base", "kb_quant_reserve", "kb_tcc_run", "kb_tcc_bootstrap_run", "kb_tcc_run_genes", "kb_tcc_run_priors", "kb_tcc_bootstrap_run_genes", "kb_eff_lens", "kb_bus_create", "kb_bus_batch", "kb_bus_batch_device", "kb_bus_begin_sample", "kb_bus_set_batch_barcodes", "kb_bus_lengths", "kb_bus_set_aa", "kb_bus_frame_clashes", "kb_bus_group_create", "kb_bus_group_free", "kb_bus_group_submit", "kb_bus_group_complete", "kb_bus_group_begin_sample", "kb_bus_group_finalize", "kb_bus_group_ec_table", "kb_bus_group_lengths", "kb_bus_group_frame_clashes", "kb_fastx_summary", "kb_fastx_summary_mt", "kb_gz_summary", "kb_counts_to_tpm",
 ]
 
 # kb_tcc_bootstrap_cb: (user, first problem, count, est_counts, rounds, resampled counts or NULL) -> 0 to go on
@@ -183,6 +184,15 @@ def lib():
     L.kb_bus_set_batch_barcodes.argtypes = [vp, C.c_int32]
     L.kb_bus_set_aa.argtypes = [vp, C.c_int32]
     L.kb_bus_frame_clashes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.kb_bus_group_create.argtypes = [vp, i32, C.POINTER(vp)]
+    L.kb_bus_group_free.argtypes = [vp]
+    L.kb_bus_group_submit.argtypes = [vp, i32, vp, vp, u32, C.POINTER(u64)]
+    L.kb_bus_group_complete.argtypes = [vp, u64, vp, C.POINTER(u32)]
+    L.kb_bus_group_begin_sample.argtypes = [vp, u64]
+    L.kb_bus_group_finalize.argtypes = [vp, C.POINTER(kb_run_stats)]
+    L.kb_bus_group_ec_table.argtypes = [vp, vp, vp, vp]
+    L.kb_bus_group_lengths.argtypes = [vp, vp, vp]
+    L.kb_bus_group_frame_clashes.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.kb_fastx_summary.argtypes = [C.c_char_p, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     L.kb_gz_summary.argtypes = [C.c_char_p, C.POINTER(u64), C.POINTER(C.c_uint32)]
     L.kb_fastx_summary_mt.argtypes = [C.c_char_p, C.c_int, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
@@ -534,6 +544,86 @@ class BUSProcessor(MinCollector):
         """--aa: the run's frame clashes ("n_frame_clashes" of run_info.json)."""
         n = C.c_uint64(0)
         _ck(lib().kb_bus_frame_clashes(self._h, C.byref(n)))
+        return n.value
+
+
+class BUSGroup:
+    """`bus --devices` (kb_bus_group_*): batches of one read stream dealt to several fresh BUSProcessor runs with the same
+    options (one index replica each), records and EC table numbered as one run fed the whole stream would number them.
+    Batches complete in submission order; fragment lengths are member 0's."""
+
+    def __init__(self, members):
+        self.members = list(members)
+        arr = (C.c_void_p * len(self.members))(*[m._h.value for m in self.members])
+        self._h = C.c_void_p()
+        _ck(lib().kb_bus_group_create(arr, len(self.members), C.byref(self._h)))
+        self._pending = {}          # ticket -> number of read sets (the capacity of its records)
+        self._stats = None
+
+    def close(self):
+        if self._h:
+            lib().kb_bus_group_free(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def submit(self, member, files):
+        """files: (bases uint8, offsets uint32) per file of the technology, as BUSProcessor.process_sets -> ticket"""
+        nf = self.members[member].nfiles if 0 <= member < len(self.members) else len(files)
+        bs = [np.ascontiguousarray(b, np.uint8) for b, _ in files]
+        os_ = [np.ascontiguousarray(o, np.uint32) for _, o in files]
+        n = len(os_[0]) - 1
+        bp = (C.c_void_p * nf)(*[b.ctypes.data for b in bs])
+        op = (C.c_void_p * nf)(*[o.ctypes.data for o in os_])
+        t = C.c_uint64(0)
+        _ck(lib().kb_bus_group_submit(self._h, member, bp, op, n, C.byref(t)))
+        self._pending[t.value] = n
+        self._stats = None
+        return t.value
+
+    def complete(self, ticket):
+        """-> the batch's records (structured array), run-wide EC ids"""
+        rec = np.zeros(max(1, self._pending.get(ticket, 0)), BUS_RECORD_DTYPE)
+        nrec = C.c_uint32(0)
+        _ck(lib().kb_bus_group_complete(self._h, C.c_uint64(ticket), _p(rec), C.byref(nrec)))
+        self._pending.pop(ticket, None)
+        return rec[: nrec.value]
+
+    def begin_sample(self, barcode):
+        _ck(lib().kb_bus_group_begin_sample(self._h, C.c_uint64(barcode)))
+
+    def finalize(self):
+        s = kb_run_stats()
+        _ck(lib().kb_bus_group_finalize(self._h, C.byref(s)))
+        self._stats = {f: getattr(s, f) for f, _ in kb_run_stats._fields_}
+        return self._stats
+
+    def ec_table(self):
+        """-> (offsets uint64[n+1], tids uint32, counts uint32[n]), ids in run-wide order"""
+        st = self._stats or self.finalize()
+        n, m = st["n_ecs"], st["n_ec_entries"]
+        off = np.zeros(n + 1, np.uint64)
+        tids = np.zeros(max(1, m), np.uint32)
+        counts = np.zeros(max(1, n), np.uint32)
+        _ck(lib().kb_bus_group_ec_table(self._h, _p(off), _p(tids), _p(counts)))
+        return off, tids[:m], counts[:n]
+
+    @property
+    def flens(self):
+        return self.members[0].flens
+
+    def lengths(self):
+        b, u = np.zeros(33, np.uint32), np.zeros(33, np.uint32)
+        _ck(lib().kb_bus_group_lengths(self._h, _p(b), _p(u)))
+        return b, u
+
+    def frame_clashes(self):
+        n = C.c_uint64(0)
+        _ck(lib().kb_bus_group_frame_clashes(self._h, C.byref(n)))
         return n.value
 
 

@@ -33,6 +33,18 @@ template <class F> int guarded(F&& f) {
     return fail(KB_ERR_INDEX, e.what());
   }
 }
+
+// guarded, with the refusals of a call's preconditions (std::invalid_argument) returned as KB_ERR_INVALID
+template <class F> int guarded_invalid(F&& f) {
+  try {
+    f();
+    return KB_OK;
+  } catch (const std::invalid_argument& e) {
+    return fail(KB_ERR_INVALID, e.what());
+  } catch (...) {
+    return guarded([] { throw; });
+  }
+}
 }  // namespace
 
 struct kb_index {
@@ -41,6 +53,9 @@ struct kb_index {
 struct kb_quant {
   std::unique_ptr<kb::Quant> q;
   kb_index* owner;
+};
+struct kb_bus_group {
+  std::unique_ptr<kb::BusGroup> g;
 };
 
 extern "C" {
@@ -652,6 +667,112 @@ int kb_bus_set_aa(kb_quant* q, int32_t on) {
 int kb_bus_frame_clashes(kb_quant* q, uint64_t* n_out) {
   if (!q || !n_out) return fail(KB_ERR_INVALID, "kb_bus_frame_clashes: null argument");
   return guarded([&] { *n_out = q->q->frame_clashes(); });
+}
+
+int kb_bus_group_create(kb_quant* const* members, int32_t n, kb_bus_group** out) {
+  if (!members || !out || n < 1) return fail(KB_ERR_INVALID, "kb_bus_group_create: null argument or no members");
+  *out = nullptr;
+  std::vector<kb::Quant*> ms;
+  for (int32_t i = 0; i < n; ++i) {
+    if (!members[i]) return fail(KB_ERR_INVALID, "kb_bus_group_create: null member");
+    kb::Quant* q = members[i]->q.get();
+    for (kb::Quant* o : ms)
+      if (o == q) return fail(KB_ERR_INVALID, "kb_bus_group_create: a member is listed twice");
+    if (!q->options().bus) return fail(KB_ERR_INVALID, "kb_bus_group_create: member " + std::to_string(i) + " is not a bus run");
+    if (!q->bus_fresh()) return fail(KB_ERR_INVALID, "kb_bus_group_create: member " + std::to_string(i) + " has run a batch already");
+    ms.push_back(q);
+  }
+  const kb::Quant& a = *ms[0];
+  for (int32_t i = 1; i < n; ++i) {
+    const kb::Quant& b = *ms[i];
+    const kb::QuantOptions &x = a.options(), &y = b.options();
+    const kb::BusSpec &s = x.bus_spec, &t = y.bus_spec;
+    bool same = x.paired == y.paired && x.strand_mode == y.strand_mode && x.collect_fld == y.collect_fld &&
+                x.max_batch_reads == y.max_batch_reads && x.max_batch_bases == y.max_batch_bases && a.aa() == b.aa() &&
+                s.nfiles == t.nfiles && s.n_bc == t.n_bc && s.n_umi == t.n_umi && s.seq_file == t.seq_file &&
+                s.seq_start == t.seq_start && s.num_flag == t.num_flag && s.paired == t.paired && s.seq2_file == t.seq2_file &&
+                s.seq2_start == t.seq2_start && s.no_umi == t.no_umi && s.fake_bc == t.fake_bc && s.tag_len == t.tag_len &&
+                s.tag_bin == t.tag_bin && s.batch_bc == t.batch_bc && s.bc_prefix == t.bc_prefix;
+    for (int j = 0; j < 4; ++j)
+      same = same && s.bc_f[j] == t.bc_f[j] && s.bc_a[j] == t.bc_a[j] && s.bc_b[j] == t.bc_b[j] && s.umi_f[j] == t.umi_f[j] &&
+             s.umi_a[j] == t.umi_a[j] && s.umi_b[j] == t.umi_b[j];
+    if (!same) return fail(KB_ERR_INVALID, "kb_bus_group_create: member " + std::to_string(i) + " has other bus options than member 0");
+    kb::Index &ia = members[0]->q->index(), &ib = members[i]->q->index();
+    if (ia.flat.k != ib.flat.k || ia.flat.num_targets() != ib.flat.num_targets())
+      return fail(KB_ERR_INVALID, "kb_bus_group_create: member " + std::to_string(i) + " has an index with another k or target count");
+  }
+  return guarded([&] {
+    kb_bus_group* h = new kb_bus_group();
+    h->g.reset(new kb::BusGroup(ms));
+    *out = h;
+  });
+}
+
+void kb_bus_group_free(kb_bus_group* g) { delete g; }
+
+int kb_bus_group_submit(kb_bus_group* g, int32_t member, const char* const* bases, const uint32_t* const* offsets,
+                        uint32_t n_sets, uint64_t* ticket) {
+  if (!g || !bases || !offsets || !ticket) return fail(KB_ERR_INVALID, "kb_bus_group_submit: null argument");
+  return guarded_invalid([&] { *ticket = g->g->submit(member, bases, offsets, n_sets); });
+}
+
+int kb_bus_group_complete(kb_bus_group* g, uint64_t ticket, kb_bus_record* records_out, uint32_t* n_records_out) {
+  if (!g || !records_out) return fail(KB_ERR_INVALID, "kb_bus_group_complete: null argument");
+  return guarded_invalid([&] { g->g->complete(ticket, (kb::BusRecord*)records_out, n_records_out); });
+}
+
+int kb_bus_group_begin_sample(kb_bus_group* g, uint64_t barcode) {
+  if (!g) return fail(KB_ERR_INVALID, "kb_bus_group_begin_sample: null argument");
+  return guarded_invalid([&] { g->g->begin_sample(barcode); });
+}
+
+int kb_bus_group_finalize(kb_bus_group* g, kb_run_stats* stats) {
+  if (!g || !stats) return fail(KB_ERR_INVALID, "kb_bus_group_finalize: null argument");
+  return guarded([&] {
+    const kb::Stats s = g->g->stats();
+    const kb::EcTable& e = g->g->ec_table();
+    stats->n_processed = s.n_processed;
+    stats->n_pseudoaligned = s.n_pseudoaligned;
+    stats->n_unique = s.n_unique;
+    stats->n_ecs = e.off.size() - 1;
+    stats->n_ec_entries = e.tid.size();
+    stats->n_probes = s.n_probes;
+    stats->n_slot_visits = s.n_slot_visits;
+    stats->n_resolved = s.n_resolved;
+    stats->n_memo_hits = s.n_memo_hits;
+  });
+}
+
+int kb_bus_group_ec_table(kb_bus_group* g, uint64_t* ec_offsets, uint32_t* tids, uint32_t* counts) {
+  if (!g || !ec_offsets || !tids || !counts) return fail(KB_ERR_INVALID, "kb_bus_group_ec_table: null argument");
+  return guarded([&] {
+    const kb::EcTable& e = g->g->ec_table();
+    memcpy(ec_offsets, e.off.data(), e.off.size() * sizeof(uint64_t));
+    memcpy(tids, e.tid.data(), e.tid.size() * sizeof(uint32_t));
+    memcpy(counts, e.count.data(), e.count.size() * sizeof(uint32_t));
+  });
+}
+
+int kb_bus_group_lengths(kb_bus_group* g, uint32_t* bc_hist, uint32_t* umi_hist) {
+  if (!g || !bc_hist || !umi_hist) return fail(KB_ERR_INVALID, "kb_bus_group_lengths: null argument");
+  return guarded([&] {
+    memset(bc_hist, 0, 33 * sizeof(uint32_t));
+    memset(umi_hist, 0, 33 * sizeof(uint32_t));
+    for (int m = 0; m < g->g->n_members(); ++m) {
+      uint32_t b[33], u[33];
+      g->g->member(m).bus_lengths(b, u);
+      for (int i = 0; i < 33; ++i) { bc_hist[i] += b[i]; umi_hist[i] += u[i]; }
+    }
+  });
+}
+
+int kb_bus_group_frame_clashes(kb_bus_group* g, uint64_t* n_out) {
+  if (!g || !n_out) return fail(KB_ERR_INVALID, "kb_bus_group_frame_clashes: null argument");
+  return guarded([&] {
+    uint64_t n = 0;
+    for (int m = 0; m < g->g->n_members(); ++m) n += g->g->member(m).frame_clashes();
+    *n_out = n;
+  });
 }
 
 int kb_fastx_summary(const char* path, uint64_t* n_reads, uint64_t* n_bases, uint64_t* fnv1a) {

@@ -32,7 +32,7 @@
 #include "../../include/kallisto_b200.h"
 // Bound weakly: the command line also links against stand-ins of the library that carry only the entry points of the
 // host pipeline (tests/stub); there `quant-tcc -b`, `quant-tcc -g / -G` and --priors report the missing entry point
-// instead of failing to link; so do `bus --aa` and `bus --batch-barcodes`.
+// instead of failing to link; so do `bus --aa`, `bus --batch-barcodes` and `bus --devices`.
 #pragma weak kb_tcc_bootstrap_run
 #pragma weak kb_tcc_run_genes
 #pragma weak kb_tcc_bootstrap_run_genes
@@ -42,6 +42,15 @@
 #pragma weak kb_bus_set_aa
 #pragma weak kb_bus_set_batch_barcodes
 #pragma weak kb_bus_frame_clashes
+#pragma weak kb_bus_group_create
+#pragma weak kb_bus_group_free
+#pragma weak kb_bus_group_submit
+#pragma weak kb_bus_group_complete
+#pragma weak kb_bus_group_begin_sample
+#pragma weak kb_bus_group_finalize
+#pragma weak kb_bus_group_ec_table
+#pragma weak kb_bus_group_lengths
+#pragma weak kb_bus_group_frame_clashes
 #include "fastx.hpp"
 #include "h5_reader.hpp"
 #include "h5_writer.hpp"
@@ -641,6 +650,49 @@ class LockStep {
   size_t n_ = 0, set_ = 0;
 };
 
+// The driver initialises every VISIBLE GPU when the first CUDA call is made (about 0.1 s apiece on an 8-GPU node):
+// unless the caller set CUDA_VISIBLE_DEVICES already, only the devices this run uses are made visible, and `device` /
+// `devices` are renumbered to match.
+void restrict_visible_devices(int& device, std::vector<int>& devices) {
+  if (getenv("CUDA_VISIBLE_DEVICES")) return;
+  std::string vis;
+  if (devices.empty()) {
+    vis = std::to_string(device);
+    device = 0;
+  } else {
+    std::vector<int> uniq;                     // a device may be listed twice (two runs on one GPU)
+    for (size_t i = 0; i < devices.size(); ++i) {
+      size_t j = 0;
+      while (j < uniq.size() && uniq[j] != devices[i]) ++j;
+      if (j == uniq.size()) {
+        uniq.push_back(devices[i]);
+        vis += (vis.empty() ? "" : ",") + std::to_string(devices[i]);
+      }
+      devices[i] = (int)j;
+    }
+    device = devices[0];
+  }
+  setenv("CUDA_VISIBLE_DEVICES", vis.c_str(), 1);
+}
+
+// Loads the index once per device of `devices` (device 0 of the list first), in parallel; false after an error message
+bool load_replicas(const std::string& path, const std::vector<int>& devices, int need_positions, int threads,
+                   std::vector<kb_index*>& ixs) {
+  const int n_dev = (int)devices.size();
+  ixs.assign(n_dev, nullptr);
+  std::vector<std::string> errs(n_dev);
+  std::vector<std::thread> loaders;
+  const int lt = std::max(1, std::min(16, std::max(1, threads)) / n_dev);
+  for (int d = 0; d < n_dev; ++d)
+    loaders.emplace_back([&, d] {
+      if (kb_index_load(path.c_str(), devices[d], need_positions, lt, &ixs[d]) != KB_OK) errs[d] = kb_last_error();
+    });
+  for (auto& t : loaders) t.join();
+  for (int d = 0; d < n_dev; ++d)
+    if (!errs[d].empty()) { cerr << endl << "Error: " << errs[d] << endl; return false; }
+  return true;
+}
+
 int cmd_quant(int argc, char** argv, const std::string& call, const std::string& start_time) {
   Options opt;
   parse_quant(argc, argv, opt);
@@ -653,28 +705,7 @@ int cmd_quant(int argc, char** argv, const std::string& call, const std::string&
   std::vector<double> priors;
   if (!opt.priors.empty() && !read_priors(opt.priors, priors)) return 1;
   PhaseTimer pt;
-  // The driver initialises every VISIBLE GPU when the first CUDA call is made (about 0.1 s apiece on an 8-GPU node):
-  // unless the caller set CUDA_VISIBLE_DEVICES already, only the devices this run uses are made visible.
-  if (!getenv("CUDA_VISIBLE_DEVICES")) {
-    std::string vis;
-    if (opt.devices.empty()) {
-      vis = std::to_string(opt.device);
-      opt.device = 0;
-    } else {
-      std::vector<int> uniq;                     // a device may be listed twice (two runs on one GPU)
-      for (size_t i = 0; i < opt.devices.size(); ++i) {
-        size_t j = 0;
-        while (j < uniq.size() && uniq[j] != opt.devices[i]) ++j;
-        if (j == uniq.size()) {
-          uniq.push_back(opt.devices[i]);
-          vis += (vis.empty() ? "" : ",") + std::to_string(opt.devices[i]);
-        }
-        opt.devices[i] = (int)j;
-      }
-      opt.device = opt.devices[0];
-    }
-    setenv("CUDA_VISIBLE_DEVICES", vis.c_str(), 1);
-  }
+  restrict_visible_devices(opt.device, opt.devices);
   const bool paired = !opt.single_end;
   const size_t max_reads = 1u << 19;                 // reads per batch and mate (pinned rings: 3 x 2 x ~70 MB)
   const size_t max_bases = (size_t)max_reads * 136 + kb::FastxFile::kMaxRead;
@@ -1065,7 +1096,9 @@ void usage_bus() {
             << "    --fr-stranded / --rf-stranded / --unstranded   Strand specificity" << endl
             << "    --aa                      Align to index generated from a FASTA-file containing amino acid sequences" << endl
             << "                              (single-end reads; not with --tag or an index with a D-list)" << endl
-            << "    --device=INT              CUDA device ordinal (default: 0)" << endl;
+            << "    --device=INT              CUDA device ordinal (default: 0)" << endl
+            << "    --devices=LIST            Comma-separated CUDA devices (a device may be listed twice): batches of" << endl
+            << "                              read sets are dealt to all of them; output as with one device" << endl;
 }
 
 int cmd_bus(int argc, char** argv, const std::string& call, const std::string& start_time) {
@@ -1092,13 +1125,28 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
                                          {"technology", required_argument, 0, 'x'},
                                          {"threads", required_argument, 0, 't'},
                                          {"device", required_argument, 0, 'D'},
+                                         {"devices", required_argument, 0, 'G'},
                                          {0, 0, 0, 0}};
   int c, oi = 0;
+  bool bad_devices = false;
   while ((c = getopt_long(argc, argv, opt_string, long_options, &oi)) != -1) {
     switch (c) {
       case 'i': opt.index = optarg; break;
       case 'o': opt.output = optarg; break;
       case 'x': technology = optarg; break;
+      case 'G': {
+        std::stringstream ss(optarg);
+        std::string tok;
+        opt.devices.clear();
+        while (std::getline(ss, tok, ',')) {
+          int v = -1;
+          const auto r = std::from_chars(tok.data(), tok.data() + tok.size(), v);
+          if (r.ec != std::errc() || r.ptr != tok.data() + tok.size() || v < 0) bad_devices = true;
+          opt.devices.push_back(v);
+        }
+        if (opt.devices.empty()) bad_devices = true;
+        break;
+      }
       case 't': std::stringstream(optarg) >> opt.threads; break;
       case 'n': num_flag = 1; break;
       case 'D': std::stringstream(optarg) >> opt.device; break;
@@ -1108,10 +1156,12 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
     }
   }
   for (int i = optind; i < argc; i++) opt.files.push_back(argv[i]);
+  if (!opt.devices.empty()) opt.device = opt.devices[0];
   // ---- CheckOptionsBus
   bool ret = true;
   struct stat stt;
   cerr << endl;
+  if (bad_devices) { cerr << "Error: --devices needs a comma-separated list of device ordinals (e.g. 0,1 or 0,0)" << endl; ret = false; }
   if (opt.index.empty()) { cerr << ERROR_STR << " kallisto index file missing" << endl; ret = false; }
   else if (stat(opt.index.c_str(), &stt) != 0) { cerr << ERROR_STR << " kallisto index file not found " << opt.index << endl; ret = false; }
   if (opt.threads <= 0) { cerr << "Error: invalid number of threads " << opt.threads << endl; ret = false; }
@@ -1362,12 +1412,27 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   else if (stat(opt.output.c_str(), &stt) == 0) {
     if (!S_ISDIR(stt.st_mode)) { cerr << "Error: file " << opt.output << " exists and is not a directory" << endl; ret = false; }
   } else if (ret && mkdir(opt.output.c_str(), 0777) == -1) { cerr << "Error: could not create directory " << opt.output << endl; ret = false; }
+  // --devices with two entries or more: one run per entry, one index replica each, driven as a kb_bus_group
+  const int n_dev = opt.devices.size() > 1 ? (int)opt.devices.size() : 1;
+  if (ret && n_dev > 1 &&
+      (!kb_bus_group_create || !kb_bus_group_free || !kb_bus_group_submit || !kb_bus_group_complete || !kb_bus_group_begin_sample ||
+       !kb_bus_group_finalize || !kb_bus_group_ec_table || !kb_bus_group_lengths || !kb_bus_group_frame_clashes)) {
+    cerr << "Error: this libkallisto_b200 has no kb_bus_group_create (bus --devices)" << endl;
+    return 1;
+  }
   if (!ret) {
     usage_bus();
     return 1;
   }
   kb_index* ix = nullptr;
-  KB_TRY(kb_index_load(opt.index.c_str(), opt.device, 0, std::min(16, std::max(1, opt.threads)), &ix));
+  std::vector<kb_index*> ixs;
+  if (n_dev > 1) {
+    restrict_visible_devices(opt.device, opt.devices);
+    if (!load_replicas(opt.index, opt.devices, 0, opt.threads, ixs)) return 1;
+    ix = ixs[0];
+  } else {
+    KB_TRY(kb_index_load(opt.index.c_str(), opt.device, 0, std::min(16, std::max(1, opt.threads)), &ix));
+  }
   kb_index_info info;
   kb_index_get_info(ix, &info);
   cerr << "[index] k-mer length: " << info.k << endl;
@@ -1385,17 +1450,23 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   bo.max_batch_sets = (uint32_t)max_reads;
   bo.max_batch_bases = 2 * max_bases;
   kb_quant* q = nullptr;
-  KB_TRY(kb_bus_create(ix, &bo, &q));
-  if (aa_flag) {
-    if (!kb_bus_set_aa || !kb_bus_frame_clashes) { cerr << "Error: this libkallisto_b200 has no kb_bus_set_aa" << endl; return 1; }
-    KB_TRY(kb_bus_set_aa(q, 1));      // refuses an index with a D-list
-  }
   // --batch-barcodes changes nothing without --batch or with -x bulk (src/main.cpp:2409, src/ProcessReads.cpp:1603-1626)
   const bool batch_barcodes = tech_batch && batch_barcodes_flag;
-  if (batch_barcodes && bo.n_bc > 0) {
-    if (!kb_bus_set_batch_barcodes) { cerr << "Error: this libkallisto_b200 has no kb_bus_set_batch_barcodes" << endl; return 1; }
-    KB_TRY(kb_bus_set_batch_barcodes(q, 1));
+  std::vector<kb_quant*> qs(n_dev, nullptr);
+  for (int d = 0; d < n_dev; ++d) {
+    KB_TRY(kb_bus_create(n_dev > 1 ? ixs[d] : ix, &bo, &qs[d]));
+    if (aa_flag) {
+      if (!kb_bus_set_aa || !kb_bus_frame_clashes) { cerr << "Error: this libkallisto_b200 has no kb_bus_set_aa" << endl; return 1; }
+      KB_TRY(kb_bus_set_aa(qs[d], 1));      // refuses an index with a D-list
+    }
+    if (batch_barcodes && bo.n_bc > 0) {
+      if (!kb_bus_set_batch_barcodes) { cerr << "Error: this libkallisto_b200 has no kb_bus_set_batch_barcodes" << endl; return 1; }
+      KB_TRY(kb_bus_set_batch_barcodes(qs[d], 1));
+    }
   }
+  q = qs[0];
+  kb_bus_group* grp = nullptr;
+  if (n_dev > 1) KB_TRY(kb_bus_group_create(qs.data(), n_dev, &grp));
   auto spec_len = [](const kb_bus_substr* v, int n) {   // BUSOptions::getBCLength / getUMILength
     int r = 0;
     for (int i = 0; i < n; ++i) {
@@ -1443,6 +1514,26 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   const size_t n_samples = (by_sample && !interleaved_flag) ? std::max<size_t>(1, opt.files.size() / (size_t)bo.nfiles) : 1;
   std::vector<std::vector<uint32_t>> sample_flens(n_samples, std::vector<uint32_t>(1000, 0));
   size_t cur_sample = (size_t)-1;
+  // --devices: the outstanding batches (ticket, member), oldest first; records are written in ticket order, so
+  // output.bus is the one-device file
+  std::vector<std::pair<uint64_t, int>> outstanding;
+  std::vector<char> busy(n_dev, 0);
+  auto complete_oldest = [&]() {
+    uint32_t nrec = 0;
+    const std::pair<uint64_t, int> t = outstanding.front();
+    outstanding.erase(outstanding.begin());
+    busy[t.second] = 0;
+    KB_TRY(kb_bus_group_complete(grp, t.first, recs.data(), &nrec));
+    busf.write((const char*)recs.data(), (std::streamsize)nrec * sizeof(kb_bus_record));
+  };
+  auto drain = [&]() {
+    while (!outstanding.empty()) complete_oldest();
+  };
+  // Paired runs sample fragment lengths from the first 10000 qualifying pairs of each sample: member 0 takes the
+  // sample's batches, one at a time, until its histogram holds them; after that (and in unpaired runs from the start)
+  // batches are dealt round-robin, one per member in flight.
+  bool fld_done = !bo.paired;
+  size_t rr = 0;
   {
     LockStep ls(streams);
     const char* bp[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1454,16 +1545,43 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
         // from 0; its id is the fake barcode of its records without a technology or, with --batch-barcodes, goes into
         // the barcode; a technology without a barcode read gives 16 x 'A' otherwise (src/ProcessReads.cpp:371-404,
         // 486-493,1583-1627)
+        if (grp) drain();
         if (cur_sample != (size_t)-1) KB_TRY(kb_quant_get_flens(q, sample_flens[cur_sample].data()));
         cur_sample = ls.file_set();
         const uint64_t id = sample_barcode.empty() ? (uint64_t)cur_sample : sample_barcode[cur_sample];
-        KB_TRY(kb_bus_begin_sample(q, (tech_batch && !batch_barcodes && bo.n_bc == 0) ? 0 : id));
+        const uint64_t bc = (tech_batch && !batch_barcodes && bo.n_bc == 0) ? 0 : id;
+        if (grp) {
+          KB_TRY(kb_bus_group_begin_sample(grp, bc));
+          fld_done = !bo.paired;
+          rr = 0;
+        } else {
+          KB_TRY(kb_bus_begin_sample(q, bc));
+        }
       }
-      uint32_t nrec = 0;
-      KB_TRY(kb_bus_batch(q, bp, op, (uint32_t)n, recs.data(), &nrec));
-      busf.write((const char*)recs.data(), (std::streamsize)nrec * sizeof(kb_bus_record));
-      ls.release();
+      if (!grp) {
+        uint32_t nrec = 0;
+        KB_TRY(kb_bus_batch(q, bp, op, (uint32_t)n, recs.data(), &nrec));
+        busf.write((const char*)recs.data(), (std::streamsize)nrec * sizeof(kb_bus_record));
+        ls.release();
+        continue;
+      }
+      const int m = fld_done ? (int)(rr++ % (size_t)n_dev) : 0;
+      while (busy[m]) complete_oldest();
+      uint64_t ticket = 0;
+      KB_TRY(kb_bus_group_submit(grp, m, bp, op, (uint32_t)n, &ticket));
+      outstanding.push_back({ticket, m});
+      busy[m] = 1;
+      ls.release();      // the batch is on the device: the parsers may refill its ring slots
+      if (!fld_done) {
+        drain();
+        uint32_t fl[1000];
+        KB_TRY(kb_quant_get_flens(q, fl));
+        uint64_t cnt = 0;
+        for (int i = 0; i < 1000; ++i) cnt += fl[i];
+        fld_done = cnt >= 10000;
+      }
     }
+    if (grp) drain();
   }
   for (auto& t : readers) t.join();
   busf.close();
@@ -1498,7 +1616,8 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   // batch run
   if (!by_sample) {
     uint32_t bh[33], uh[33];
-    KB_TRY(kb_bus_lengths(q, bh, uh));
+    if (grp) KB_TRY(kb_bus_group_lengths(grp, bh, uh));
+    else KB_TRY(kb_bus_lengths(q, bh, uh));
     uint32_t bl = 0, ul = 0;
     for (uint32_t i = 0; i <= 32; ++i) {
       if (bh[i] > bh[bl]) bl = i;
@@ -1520,14 +1639,16 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
     }
   }
   kb_run_stats st{};
-  KB_TRY(kb_quant_finalize(q, &st));
+  if (grp) KB_TRY(kb_bus_group_finalize(grp, &st));
+  else KB_TRY(kb_quant_finalize(q, &st));
   cerr << "[quant] processed " << pretty_num(st.n_processed) << " reads, " << pretty_num(st.n_pseudoaligned)
        << " reads pseudoaligned" << endl;
   if (st.n_pseudoaligned == 0) cerr << "[~warn] no reads pseudoaligned." << endl;
   {   // writeECList, src/PlaintextWriter.cpp:235-266
     std::vector<uint64_t> eo(st.n_ecs + 1);
     std::vector<uint32_t> et(std::max<uint64_t>(1, st.n_ec_entries)), ec(std::max<uint64_t>(1, st.n_ecs));
-    KB_TRY(kb_quant_ec_table(q, eo.data(), et.data(), ec.data(), nullptr));
+    if (grp) KB_TRY(kb_bus_group_ec_table(grp, eo.data(), et.data(), ec.data()));
+    else KB_TRY(kb_quant_ec_table(q, eo.data(), et.data(), ec.data(), nullptr));
     std::ofstream ecof(opt.output + "/matrix.ec");
     for (uint64_t i = 0; i < st.n_ecs; ++i) {
       ecof << i << "\t";
@@ -1542,7 +1663,8 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   std::string frame_clashes;
   if (aa_flag) {
     uint64_t nc = 0;
-    KB_TRY(kb_bus_frame_clashes(q, &nc));
+    if (grp) KB_TRY(kb_bus_group_frame_clashes(grp, &nc));
+    else KB_TRY(kb_bus_frame_clashes(q, &nc));
     frame_clashes = std::to_string(nc);
   }
   write_run_info(opt.output + "/run_info.json", info.n_targets, 0, st.n_processed, st.n_pseudoaligned, st.n_unique, 13, info.k,
@@ -1550,8 +1672,12 @@ int cmd_bus(int argc, char** argv, const std::string& call, const std::string& s
   cerr << endl;
   if (!getenv("KB_CLI_CLEANUP")) finish(st.n_pseudoaligned == 0 ? 1 : 0);
   free_streams(streams);
-  kb_quant_free(q);
-  kb_index_free(ix);
+  if (grp) kb_bus_group_free(grp);
+  for (kb_quant* m : qs) kb_quant_free(m);
+  if (n_dev > 1)
+    for (kb_index* x : ixs) kb_index_free(x);
+  else
+    kb_index_free(ix);
   return st.n_pseudoaligned == 0 ? 1 : 0;
 }
 

@@ -438,6 +438,7 @@ Quant::~Quant() {
   if (stream_) cudaStreamSynchronize(stream_);
   if (own_ws_) { delete emws_; delete bws_; } else { ix_.ws_in_use = false; }
   if (h_off_pinned_) cudaFreeHost(h_off_pinned_);
+  if (h_grp_) cudaFreeHost(h_grp_);
   for (auto ev : events_) cudaEventDestroy(ev);
   for (int i = 0; i < 2; ++i) {
     if (ev_copied_[i]) cudaEventDestroy(ev_copied_[i]);
@@ -720,20 +721,108 @@ void Quant::bus_batch_host(const char* const* bases, const uint32_t* const* offs
   if (!opt_.bus) throw Error("kallisto_b200: not a bus run");
   if (n_records_out) *n_records_out = 0;
   if (n_sets == 0) return;
+  if (grp_pending_) throw Error("kallisto_b200: this bus run has a group batch outstanding");
+  Staged g{};
+  const uint32_t maxlen = bus_stage(bases, offs, n_sets, g);
+  const uint32_t n_rec = bus_core(g.bases, g.off, n_sets, maxlen);
+  if (n_rec && records_out) {
+    bus_rec_.download(records_out, n_rec, 0, stream_);
+    KB_CK(cudaStreamSynchronize(stream_));
+  }
+  if (n_records_out) *n_records_out = n_rec;
+}
+
+uint32_t Quant::bus_stage(const char* const* bases, const uint32_t* const* offs, uint32_t n_sets, Staged& g) {
   const BusSpec& sp = opt_.bus_spec;
   for (int k = 0; k < sp.nfiles; ++k)
     if (!bases[k] || !offs[k]) throw Error("kallisto_b200: bus batch needs bases and offsets for every file of the technology");
   // This path does not overlap batches, so it stages into slot 0 only, once the run's stream is done with the batch
   // before: bus_fields, cfc_frames and pack_kernel all read the staged files, and that batch may have failed part way.
   KB_CK(cudaEventRecord(ev_done_[0], stream_));
-  const Staged g = stage(0, sp.nfiles, bases, offs, n_sets, 0, opt_.max_batch_bases / 2 + 16, (size_t)opt_.max_batch_reads + 1);
+  g = stage(0, sp.nfiles, bases, offs, n_sets, 0, opt_.max_batch_bases / 2 + 16, (size_t)opt_.max_batch_reads + 1);
   // longest cDNA read of the batch (sizes the packed-read layout)
-  const uint32_t maxlen = std::max(g.maxlen[sp.seq_file], sp.paired ? g.maxlen[sp.seq2_file] : 0u);
-  const uint32_t n_rec = bus_core(g.bases, g.off, n_sets, maxlen);
-  if (n_rec && records_out) {
-    bus_rec_.download(records_out, n_rec, 0, stream_);
-    KB_CK(cudaStreamSynchronize(stream_));
+  return std::max(g.maxlen[sp.seq_file], sp.paired ? g.maxlen[sp.seq2_file] : 0u);
+}
+
+void Quant::bus_group_submit(const char* const* bases, const uint32_t* const* offs, uint32_t n_sets, uint64_t base,
+                             uint64_t sample_base) {
+  KB_CK(cudaSetDevice(ix_.device));
+  if (!opt_.bus) throw Error("kallisto_b200: not a bus run");
+  if (grp_pending_) throw Error("kallisto_b200: this group member has a batch outstanding");
+  grp_n_ = n_sets;
+  if (n_sets == 0) { grp_pending_ = true; return; }
+  Staged g{};
+  const uint32_t maxlen = bus_stage(bases, offs, n_sets, g);
+  set_frag_base(base);                       // run_batch's first-occurrence keys: the run-wide index too
+  grp_handles_ = bus_enqueue(g.bases, g.off, n_sets, maxlen, base, base - sample_base);
+  cudaStream_t st = stream_;
+  const size_t n1 = (size_t)n_sets + 1;
+  auto grow = [&](auto& b, size_t need) { if (b.n < need) b.alloc(std::max<size_t>(need, (size_t)opt_.max_batch_reads + 1)); };
+  grow(grp_len_, n1); grow(grp_eoff_, n1); grow(grp_off_, n1); grow(grp_tid_, 1);
+  if (!h_grp_) KB_CK(cudaMallocHost((void**)&h_grp_, 8 * sizeof(unsigned long long)));
+  launch_bus_new_sets(dd_, grp_handles_, n_sets, base, bus_isnew_.p, bus_newrank_.p, bus_ismapped_.p, bus_rank_.p,
+                      grp_len_.p, grp_eoff_.p, (uint32_t)std::min<size_t>(grp_tid_.n, 0xFFFFFFFFu), grp_off_.p, grp_tid_.p,
+                      bus_tmp_.p, bus_tmp_.n, st);
+  KB_CK(cudaGetLastError());
+  n_kernel_launches += 4;      // bus_fields, bus_newflag, bus_newlen, bus_export
+  // the batch's totals, read by bus_group_new_sets: n_new, entries, records, valid sets, long barcodes
+  uint32_t* h32 = reinterpret_cast<uint32_t*>(h_grp_);
+  KB_CK(cudaMemcpyAsync(h32 + 0, bus_newrank_.p + n_sets, 4, cudaMemcpyDeviceToHost, st));
+  KB_CK(cudaMemcpyAsync(h32 + 1, grp_eoff_.p + n_sets, 4, cudaMemcpyDeviceToHost, st));
+  KB_CK(cudaMemcpyAsync(h32 + 2, bus_rank_.p + n_sets, 4, cudaMemcpyDeviceToHost, st));
+  KB_CK(cudaMemcpyAsync(h_grp_ + 2, bus_nvalid_.p, 16, cudaMemcpyDeviceToHost, st));
+  grp_pending_ = true;
+  // the caller may reuse its buffers once the copy is done; the kernels keep running
+  KB_CK(cudaEventSynchronize(ev_copied_[0]));
+}
+
+void Quant::bus_group_new_sets(std::vector<uint32_t>& off, std::vector<uint32_t>& tids) {
+  if (!grp_pending_) throw Error("kallisto_b200: no group batch outstanding on this member");
+  off.assign(1, 0);
+  tids.clear();
+  if (grp_n_ == 0) return;
+  KB_CK(cudaSetDevice(ix_.device));
+  cudaStream_t st = stream_;
+  KB_CK(cudaStreamSynchronize(st));
+  const uint32_t* h32 = reinterpret_cast<const uint32_t*>(h_grp_);
+  const uint32_t n_new = h32[0], n_ent = h32[1];
+  if (h_grp_[3]) {
+    grp_pending_ = false;
+    throw Error("kallisto_b200: --batch-barcodes: " + std::to_string(h_grp_[3]) + " read set(s) of this batch have a barcode of "
+                "more than 32 letters, which cannot take the sample's number in front of it");
   }
+  if (n_ent > grp_tid_.n) {       // the first gather ran out of room: gather again into a buffer of the right size
+    grp_tid_.alloc((size_t)n_ent + n_ent / 4);
+    launch_bus_export_gather(dd_, grp_handles_, grp_n_, bus_isnew_.p, bus_newrank_.p, grp_eoff_.p,
+                             (uint32_t)std::min<size_t>(grp_tid_.n, 0xFFFFFFFFu), grp_off_.p, grp_tid_.p, st);
+    KB_CK(cudaGetLastError());
+    ++n_kernel_launches;
+  }
+  off.resize((size_t)n_new + 1);
+  tids.resize(n_ent);
+  grp_off_.download(off.data(), (size_t)n_new + 1, 0, st);
+  if (n_ent) grp_tid_.download(tids.data(), n_ent, 0, st);
+  KB_CK(cudaStreamSynchronize(st));
+}
+
+void Quant::bus_group_finish(const int32_t* gid, BusRecord* records_out, uint32_t* n_records_out) {
+  if (!grp_pending_) throw Error("kallisto_b200: no group batch outstanding on this member");
+  grp_pending_ = false;
+  if (n_records_out) *n_records_out = 0;
+  if (grp_n_ == 0) return;
+  KB_CK(cudaSetDevice(ix_.device));
+  cudaStream_t st = stream_;
+  const uint32_t* h32 = reinterpret_cast<const uint32_t*>(h_grp_);
+  const uint32_t n_new = h32[0], n_rec = h32[2];
+  grp_gid_.grow(std::max<size_t>(1, n_new), 0.25);
+  if (n_new) grp_gid_.upload(gid, n_new, st);
+  launch_bus_group_records(grp_handles_, grp_n_, bus_isnew_.p, bus_newrank_.p, grp_gid_.p, bus_idof_.p, bus_ismapped_.p,
+                           bus_rank_.p, (const uint64_t*)bus_bc_.p, (const uint64_t*)bus_umi_.p, bus_flags_.p, bus_rec_.p, st);
+  KB_CK(cudaGetLastError());
+  n_kernel_launches += 2;      // bus_newid_gid, bus_records
+  if (n_rec && records_out) bus_rec_.download(records_out, n_rec, 0, st);
+  KB_CK(cudaStreamSynchronize(st));
+  bus_valid_total_ += h_grp_[2];
   if (n_records_out) *n_records_out = n_rec;
 }
 
@@ -750,6 +839,31 @@ uint32_t Quant::bus_batch_device(const uint8_t* const* d_bases, const uint32_t* 
 }
 
 uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, uint32_t n_sets, uint32_t maxlen) {
+  cudaStream_t st = stream_;
+  const uint64_t base = n_frag_total_;
+  // --num: read numbers restart with every sample (one reader per batch)
+  const int32_t* handles = bus_enqueue(db, dofs, n_sets, maxlen, base, n_frag_total_ - bus_sample_base_);
+  launch_bus_records(dd_, handles, n_sets, base, bus_next_id_, bus_idof_.p, bus_isnew_.p, bus_newrank_.p,
+                     bus_ismapped_.p, bus_rank_.p, (const uint64_t*)bus_bc_.p, (const uint64_t*)bus_umi_.p, bus_flags_.p,
+                     bus_rec_.p, bus_tmp_.p, bus_tmp_.n, st);
+  KB_CK(cudaGetLastError());
+  n_kernel_launches += 4;      // bus_fields, bus_newflag, bus_newid, bus_records (CUB scans not counted)
+  uint32_t n_new = 0, n_rec = 0;
+  unsigned long long n_valid[2] = {0, 0};
+  bus_newrank_.download(&n_new, 1, n_sets, st);
+  bus_rank_.download(&n_rec, 1, n_sets, st);
+  bus_nvalid_.download(n_valid, 2, 0, st);
+  KB_CK(cudaStreamSynchronize(st));
+  if (n_valid[1])
+    throw Error("kallisto_b200: --batch-barcodes: " + std::to_string(n_valid[1]) + " read set(s) of this batch have a barcode of "
+                "more than 32 letters, which cannot take the sample's number in front of it");
+  bus_next_id_ += n_new;
+  bus_valid_total_ += n_valid[0];
+  return n_rec;
+}
+
+const int32_t* Quant::bus_enqueue(const uint8_t* const* db, const uint32_t* const* dofs, uint32_t n_sets, uint32_t maxlen,
+                                  uint64_t base, uint64_t set_base) {
   const BusSpec& sp = opt_.bus_spec;
   cudaStream_t st = stream_;
   BusArgs a{};
@@ -766,7 +880,7 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   if (bus_tmp_.n < tb) bus_tmp_.alloc(std::max(tb, bus_scan_bytes(opt_.max_batch_reads)));
   bus_nvalid_.zero(st);
   a.n_sets = n_sets;
-  a.set_base = n_frag_total_ - bus_sample_base_;      // --num: read numbers restart with every sample (one reader per batch)
+  a.set_base = set_base;
   a.spec = sp;
   a.barcode = (uint64_t*)bus_bc_.p; a.umi = (uint64_t*)bus_umi_.p; a.flags = bus_flags_.p; a.skip = bus_skip_.p;
   a.notag = sp.tag_len ? bus_notag_.p : nullptr;
@@ -790,7 +904,6 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
     min_start = std::min(min_start, sp.paired ? std::min(in.alt_start, in.alt_start2) : in.alt_start);
   }
   maxlen = maxlen > min_start ? maxlen - min_start : 1;
-  const uint64_t base = n_frag_total_;
   if (aa_) {
     // the six reading frames of every set in comma-free code (kernels_cfc.cu), 6 n_sets unpaired fragments; a skipped
     // set has empty frames
@@ -835,24 +948,7 @@ uint32_t Quant::bus_core(const uint8_t* const* db, const uint32_t* const* dofs, 
   // the records need the whole batch, and the batch's read-set fields (barcodes, skip and tag marks) are rewritten by
   // the next one: this path does not overlap batches
   join();
-  const int32_t* handles = aa_ ? cfc_handles_.p : bws_->slot[last_slot_].d_handles.p;
-  launch_bus_records(dd_, handles, n_sets, base, bus_next_id_, bus_idof_.p, bus_isnew_.p, bus_newrank_.p,
-                     bus_ismapped_.p, bus_rank_.p, (const uint64_t*)bus_bc_.p, (const uint64_t*)bus_umi_.p, bus_flags_.p,
-                     bus_rec_.p, bus_tmp_.p, bus_tmp_.n, st);
-  KB_CK(cudaGetLastError());
-  n_kernel_launches += 4;      // bus_fields, bus_newflag, bus_newid, bus_records (CUB scans not counted)
-  uint32_t n_new = 0, n_rec = 0;
-  unsigned long long n_valid[2] = {0, 0};
-  bus_newrank_.download(&n_new, 1, n_sets, st);
-  bus_rank_.download(&n_rec, 1, n_sets, st);
-  bus_nvalid_.download(n_valid, 2, 0, st);
-  KB_CK(cudaStreamSynchronize(st));
-  if (n_valid[1])
-    throw Error("kallisto_b200: --batch-barcodes: " + std::to_string(n_valid[1]) + " read set(s) of this batch have a barcode of "
-                "more than 32 letters, which cannot take the sample's number in front of it");
-  bus_next_id_ += n_new;
-  bus_valid_total_ += n_valid[0];
-  return n_rec;
+  return aa_ ? cfc_handles_.p : bws_->slot[last_slot_].d_handles.p;
 }
 
 void Quant::bus_begin_sample(uint64_t barcode) {
@@ -926,6 +1022,92 @@ void Quant::bus_lengths(uint32_t* bc_hist, uint32_t* umi_hist) {
   }
   memcpy(bc_hist, h, 33 * 4);
   memcpy(umi_hist, h + 33, 33 * 4);
+}
+
+BusGroup::BusGroup(std::vector<Quant*> members) : m_(std::move(members)), busy_(m_.size(), false) {
+  table_.off.assign(1, 0);
+}
+
+uint64_t BusGroup::submit(int member, const char* const* bases, const uint32_t* const* offs, uint32_t n_sets) {
+  if (member < 0 || member >= (int)m_.size()) throw std::invalid_argument("kb_bus_group_submit: no such member");
+  if (busy_[member]) throw std::invalid_argument("kb_bus_group_submit: the member has a batch outstanding; complete it first");
+  // every member numbers read sets run-wide: the dictionary's first-occurrence keys and --num read numbers
+  m_[member]->bus_group_submit(bases, offs, n_sets, n_sets_total_, sample_base_);
+  busy_[member] = true;
+  queue_.push_back(member);
+  n_sets_total_ += n_sets;
+  return next_ticket_++;
+}
+
+// The commit rule.  A set that is new run-wide in this batch is, among the sets new run-wide, in order of first
+// occurrence within the batch, and it is new on the member too (an earlier batch on the member would have committed
+// it); a set the member saw before keeps the id an earlier batch committed.  So handing out the next ids in the
+// member's new_rank order, after every earlier ticket, gives the ids of one run fed the whole stream.
+void BusGroup::complete(uint64_t ticket, BusRecord* records_out, uint32_t* n_records_out) {
+  if (queue_.empty()) throw std::invalid_argument("kb_bus_group_complete: no batch outstanding");
+  if (ticket != done_tickets_)
+    throw std::invalid_argument("kb_bus_group_complete: ticket " + std::to_string(ticket) + " is not the oldest outstanding batch (" +
+                                std::to_string(done_tickets_) + ")");
+  const int d = queue_.front();
+  queue_.erase(queue_.begin());
+  busy_[d] = false;
+  ++done_tickets_;
+  Quant& q = *m_[d];
+  std::vector<uint32_t> off, tids;
+  q.bus_group_new_sets(off, tids);
+  const size_t n_new = off.size() - 1;
+  std::vector<int32_t> gid(n_new);
+  std::vector<uint32_t> key;
+  for (size_t i = 0; i < n_new; ++i) {
+    key.assign(tids.begin() + off[i], tids.begin() + off[i + 1]);
+    auto it = reg_.find(key);
+    if (it == reg_.end()) {
+      const int32_t id = (int32_t)(table_.off.size() - 1);
+      table_.tid.insert(table_.tid.end(), key.begin(), key.end());
+      table_.off.push_back(table_.tid.size());
+      it = reg_.emplace(std::move(key), id).first;
+      key = std::vector<uint32_t>();
+    }
+    gid[i] = it->second;
+  }
+  q.bus_group_finish(gid.data(), records_out, n_records_out);
+}
+
+void BusGroup::begin_sample(uint64_t barcode) {
+  if (!queue_.empty()) throw std::invalid_argument("kb_bus_group_begin_sample: complete the outstanding batches first");
+  for (Quant* q : m_) q->bus_begin_sample(barcode);
+  sample_base_ = n_sets_total_;
+}
+
+const EcTable& BusGroup::ec_table() {
+  const size_t n = table_.off.size() - 1;
+  table_.count.assign(n, 0);
+  std::vector<uint32_t> key;
+  for (Quant* q : m_) {
+    const EcTable& e = q->finalize_ecs();
+    for (uint32_t i = 0; i < e.n(); ++i) {
+      key.assign(e.tid.begin() + e.off[i], e.tid.begin() + e.off[i + 1]);
+      auto it = reg_.find(key);
+      if (it == reg_.end()) throw Error("kallisto_b200: a member's equivalence class was never committed to its group");
+      table_.count[it->second] += e.count[i];
+    }
+  }
+  return table_;
+}
+
+Stats BusGroup::stats() {
+  Stats s;
+  for (Quant* q : m_) {
+    const Stats t = q->stats();
+    s.n_processed += t.n_processed;
+    s.n_pseudoaligned += t.n_pseudoaligned;
+    s.n_unique += t.n_unique;
+    s.n_probes += t.n_probes;
+    s.n_slot_visits += t.n_slot_visits;
+    s.n_resolved += t.n_resolved;
+    s.n_memo_hits += t.n_memo_hits;
+  }
+  return s;
 }
 
 void Quant::set_flens(const uint32_t* f) {

@@ -14,6 +14,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "index_v13.hpp"
@@ -248,6 +249,18 @@ class Quant {
   void set_aa(bool on);
   // cardinality_clashes of the run: frames whose set was as small as the winning frame's before them
   uint64_t frame_clashes();
+  // ---- `bus --devices`: this run as a member of a BusGroup (several runs, one run-wide EC numbering) ----
+  // Stages one batch whose first read set has the run-wide index `base`, in a sample whose first read set has the
+  // run-wide index `sample_base`, and enqueues its work up to the export of the sets new on this run.  Returns once
+  // the host buffers may be reused.  One batch at a time: bus_group_finish ends it.
+  void bus_group_submit(const char* const* bases, const uint32_t* const* offs, uint32_t n_sets, uint64_t base,
+                        uint64_t sample_base);
+  // Waits for the submitted batch and returns its new sets in order of first occurrence (off: n_new + 1 entries)
+  void bus_group_new_sets(std::vector<uint32_t>& off, std::vector<uint32_t>& tids);
+  // Gives the new sets the run-wide ids `gid` (one per new set, in that order) and returns the batch's records
+  void bus_group_finish(const int32_t* gid, BusRecord* records_out, uint32_t* n_records_out);
+  bool bus_fresh() const { return n_frag_total_ == 0 && !grp_pending_; }
+  bool aa() const { return aa_; }
   // Same, inputs already resident in device memory; handles stay on the device
   // (device_handles(), valid until the next batch).  The call returns once the kernels are enqueued; the caller may
   // overwrite its input in the run's stream order, since that stream waits for the kernels that read it.
@@ -349,6 +362,12 @@ class Quant {
   EcNumbering number_ecs();
   void apply_l2_window();
   uint32_t bus_core(const uint8_t* const* db, const uint32_t* const* dofs, uint32_t n_sets, uint32_t maxlen);
+  // bus_core up to the records: read-set fields and pseudoalignment of a batch whose first read set has the index
+  // `base` (the dictionary's first-occurrence keys) and the read number `set_base` (--num); returns the set handles
+  const int32_t* bus_enqueue(const uint8_t* const* db, const uint32_t* const* dofs, uint32_t n_sets, uint32_t maxlen,
+                             uint64_t base, uint64_t set_base);
+  // the host batch staged for bus_enqueue (slot 0: the bus paths do not overlap batches); returns its longest cDNA read
+  uint32_t bus_stage(const char* const* bases, const uint32_t* const* offs, uint32_t n_sets, Staged& g);
 
   Index& ix_;
   QuantOptions opt_;
@@ -411,6 +430,51 @@ class Quant {
   DBuf<uint32_t> cfc_o_, cfc_set_off_, cfc_first_;
   DBuf<int32_t> cfc_handles_;
   DBuf<unsigned long long> cfc_clashes_;
+  // bus group member: the submitted batch's set handles and size, its new sets as CSR (grp_len_ / grp_eoff_: per
+  // fragment, grp_off_ / grp_tid_: per new set), the run-wide ids of those sets, and the batch's totals (pinned:
+  // n_new, total ids, records, valid sets, long barcodes)
+  bool grp_pending_ = false;
+  const int32_t* grp_handles_ = nullptr;
+  uint32_t grp_n_ = 0;
+  DBuf<uint32_t> grp_len_, grp_eoff_, grp_off_, grp_tid_;
+  DBuf<int32_t> grp_gid_;
+  unsigned long long* h_grp_ = nullptr;
+};
+
+// `bus --devices` (kb_bus_group_*): several bus runs, each on its own index replica, fed batches of one read stream,
+// whose records carry one run-wide EC numbering -- the ids of a single run fed the whole stream.  Batches complete in
+// the order they were submitted; each member's new sets are committed to a content-keyed registry (transcript list ->
+// id) on the host: a known set keeps its id, an unknown one takes the next.  One host thread drives a group.
+class BusGroup {
+ public:
+  explicit BusGroup(std::vector<Quant*> members);
+  // returns the batch's ticket; the host buffers may be reused on return
+  uint64_t submit(int member, const char* const* bases, const uint32_t* const* offs, uint32_t n_sets);
+  // the oldest outstanding batch (ticket must name it): its records with run-wide EC ids
+  void complete(uint64_t ticket, BusRecord* records_out, uint32_t* n_records_out);
+  void begin_sample(uint64_t barcode);
+  size_t outstanding() const { return queue_.size(); }
+  uint64_t n_sets_total() const { return n_sets_total_; }
+  // the run-wide table, ids in order; counts summed over the members (refreshed by every call)
+  const EcTable& ec_table();
+  Stats stats();
+  int n_members() const { return (int)m_.size(); }
+  Quant& member(int i) { return *m_[i]; }
+
+ private:
+  struct VecHash {
+    size_t operator()(const std::vector<uint32_t>& v) const {
+      uint64_t h = 1469598103934665603ULL ^ v.size();
+      for (uint32_t x : v) h = (h ^ x) * 1099511628211ULL;
+      return (size_t)h;
+    }
+  };
+  std::vector<Quant*> m_;
+  std::vector<int> queue_;          // members of the outstanding batches, oldest first
+  std::vector<bool> busy_;
+  uint64_t next_ticket_ = 0, done_tickets_ = 0, n_sets_total_ = 0, sample_base_ = 0;
+  std::unordered_map<std::vector<uint32_t>, int32_t, VecHash> reg_;
+  EcTable table_;                   // off / tid in id order; count filled by ec_table()
 };
 
 std::vector<double> mean_fl_trunc_of(const uint32_t* flens /* 1000 */, double fld_mean, double fld_sd);

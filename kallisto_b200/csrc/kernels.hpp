@@ -357,6 +357,21 @@ void launch_bus_records(const DevDict& dd, const int32_t* handle, uint32_t n, ui
                         int32_t* id_of, uint32_t* is_new, uint32_t* new_rank, uint32_t* is_mapped, uint32_t* rank,
                         const uint64_t* barcode, const uint64_t* umi, const uint32_t* flags, BusRecord* out, void* tmp,
                         size_t tmp_bytes, cudaStream_t st);
+// bus --devices (kb_bus_group_*): launch_bus_records in two halves around the host's choice of run-wide EC ids.
+// launch_bus_new_sets flags the fragments as launch_bus_records does, and lays the sets new on this run out as CSR in
+// new_rank order: out_off[0 .. n_new], out_tid[0 .. total) (ids past `cap` are left out; the total is eoff[n]).
+// len / eoff: n + 1 words each.  launch_bus_export_gather repeats the gather once the host has a large enough buffer.
+void launch_bus_new_sets(const DevDict& dd, const int32_t* handle, uint32_t n, uint64_t base, uint32_t* is_new,
+                         uint32_t* new_rank, uint32_t* is_mapped, uint32_t* rank, uint32_t* len, uint32_t* eoff,
+                         uint32_t cap, uint32_t* out_off, uint32_t* out_tid, void* tmp, size_t tmp_bytes, cudaStream_t st);
+void launch_bus_export_gather(const DevDict& dd, const int32_t* handle, uint32_t n, const uint32_t* is_new,
+                              const uint32_t* new_rank, const uint32_t* eoff, uint32_t cap, uint32_t* out_off,
+                              uint32_t* out_tid, cudaStream_t st);
+// id_of[handle] = gid[new_rank] for the new sets, then the records of launch_bus_records
+void launch_bus_group_records(const int32_t* handle, uint32_t n, const uint32_t* is_new, const uint32_t* new_rank,
+                              const int32_t* gid, int32_t* id_of, const uint32_t* is_mapped, const uint32_t* rank,
+                              const uint64_t* barcode, const uint64_t* umi, const uint32_t* flags, BusRecord* out,
+                              cudaStream_t st);
 
 // ---- translated search, bus --aa (kernels_cfc.cu) ----
 // The six reading frames of every read set in comma-free code, fragment 6 i + j = frame j of set i.

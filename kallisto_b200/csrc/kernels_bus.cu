@@ -10,6 +10,9 @@
 //                       (src/ProcessReads.cpp:603-624).
 //   bus_records_kernel  + scan: one 32-byte BUSData (src/BUSData.h:30-38) per pseudoaligned read, in
 //                       read order, ready to be appended to output.bus.
+//   bus --devices (a member of a kb_bus_group): bus_newlen_kernel + scan + bus_export_kernel lay the sets new
+//                       on the member out as CSR for the host's run-wide numbering, and bus_newid_gid_kernel
+//                       writes the ids it chose instead of next_id + rank.
 #include <cub/cub.cuh>
 
 #include "kb_device.cuh"
@@ -140,6 +143,40 @@ __global__ void bus_newid_kernel(const int32_t* handle, uint32_t n, const uint32
   if (is_new[f]) id_of[handle[f]] = (int32_t)(next_id + new_rank[f]);
 }
 
+// bus --devices: the run-wide ids of the sets new on this run, chosen by the group on the host (gid, by new_rank)
+__global__ void bus_newid_gid_kernel(const int32_t* handle, uint32_t n, const uint32_t* is_new, const uint32_t* new_rank,
+                                     const int32_t* gid, int32_t* id_of) {
+  const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= n) return;
+  if (is_new[f]) id_of[handle[f]] = gid[new_rank[f]];
+}
+
+// bus --devices: per fragment, the length of its set when the fragment is that set's first occurrence on this run
+__global__ void bus_newlen_kernel(DevDict dd, const int32_t* handle, uint32_t n, const uint32_t* is_new, uint32_t* len) {
+  const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > n) return;
+  len[f] = (f < n && is_new[f]) ? (uint32_t)((__ldcg(&dd.dslots[handle[f]]) >> 32) & 0xFFFFFFu) : 0u;
+}
+
+// bus --devices: the new sets as CSR in new_rank order (out_off: n_new + 1 entries, out_tid: their transcript ids).
+// eoff is the exclusive scan of bus_newlen_kernel's lengths over n + 1 items, so eoff[n] is the total; ids that would
+// pass `cap` are not written (the host sees the total and gathers again into a larger buffer).
+__global__ void bus_export_kernel(DevDict dd, const int32_t* handle, uint32_t n, const uint32_t* is_new,
+                                  const uint32_t* new_rank, const uint32_t* eoff, uint32_t cap, uint32_t* out_off,
+                                  uint32_t* out_tid) {
+  const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f > n) return;
+  if (f == n) { out_off[new_rank[n]] = eoff[n]; return; }
+  if (!is_new[f]) return;
+  const uint32_t o = eoff[f];
+  out_off[new_rank[f]] = o;
+  const unsigned long long word = __ldcg(&dd.dslots[handle[f]]);
+  const uint32_t l = (uint32_t)((word >> 32) & 0xFFFFFFu);
+  if ((uint64_t)o + l > cap) return;
+  const uint32_t* src = dd.pool + (uint32_t)word;
+  for (uint32_t j = 0; j < l; ++j) out_tid[o + j] = __ldcg(src + j);
+}
+
 __global__ void bus_records_kernel(const int32_t* handle, uint32_t n, const uint32_t* is_mapped, const uint32_t* rank,
                                    const int32_t* id_of, const uint64_t* barcode, const uint64_t* umi, const uint32_t* flags,
                                    BusRecord* out) {
@@ -180,6 +217,41 @@ void launch_bus_records(const DevDict& dd, const int32_t* handle, uint32_t n, ui
   cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, is_new, new_rank, (int)n + 1, st);
   cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, is_mapped, rank, (int)n + 1, st);
   bus_newid_kernel<<<g, 256, 0, st>>>(handle, n, is_new, new_rank, next_id, id_of);
+  bus_records_kernel<<<g, 256, 0, st>>>(handle, n, is_mapped, rank, id_of, barcode, umi, flags, out);
+}
+
+// bus --devices, first half: the flags and ranks of launch_bus_records, then the sets new on this run as CSR
+// (launch_bus_export_gather).  Totals land in new_rank[n] (new sets), eoff[n] (their ids) and rank[n] (records).
+void launch_bus_new_sets(const DevDict& dd, const int32_t* handle, uint32_t n, uint64_t base, uint32_t* is_new,
+                         uint32_t* new_rank, uint32_t* is_mapped, uint32_t* rank, uint32_t* len, uint32_t* eoff,
+                         uint32_t cap, uint32_t* out_off, uint32_t* out_tid, void* tmp, size_t tmp_bytes, cudaStream_t st) {
+  if (n == 0) return;
+  const unsigned g = (n + 255) / 256, g1 = (n + 256) / 256;
+  cudaMemsetAsync(is_new + n, 0, 4, st);
+  cudaMemsetAsync(is_mapped + n, 0, 4, st);
+  bus_newflag_kernel<<<g, 256, 0, st>>>(dd, handle, n, base, is_new, is_mapped);
+  cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, is_new, new_rank, (int)n + 1, st);
+  cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, is_mapped, rank, (int)n + 1, st);
+  bus_newlen_kernel<<<g1, 256, 0, st>>>(dd, handle, n, is_new, len);
+  cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, len, eoff, (int)n + 1, st);
+  launch_bus_export_gather(dd, handle, n, is_new, new_rank, eoff, cap, out_off, out_tid, st);
+}
+
+void launch_bus_export_gather(const DevDict& dd, const int32_t* handle, uint32_t n, const uint32_t* is_new,
+                              const uint32_t* new_rank, const uint32_t* eoff, uint32_t cap, uint32_t* out_off,
+                              uint32_t* out_tid, cudaStream_t st) {
+  if (n == 0) return;
+  bus_export_kernel<<<(n + 256) / 256, 256, 0, st>>>(dd, handle, n, is_new, new_rank, eoff, cap, out_off, out_tid);
+}
+
+// bus --devices, second half: the run-wide ids of the new sets (gid, n_new of them, by new_rank), then the records
+void launch_bus_group_records(const int32_t* handle, uint32_t n, const uint32_t* is_new, const uint32_t* new_rank,
+                              const int32_t* gid, int32_t* id_of, const uint32_t* is_mapped, const uint32_t* rank,
+                              const uint64_t* barcode, const uint64_t* umi, const uint32_t* flags, BusRecord* out,
+                              cudaStream_t st) {
+  if (n == 0) return;
+  const unsigned g = (n + 255) / 256;
+  bus_newid_gid_kernel<<<g, 256, 0, st>>>(handle, n, is_new, new_rank, gid, id_of);
   bus_records_kernel<<<g, 256, 0, st>>>(handle, n, is_mapped, rank, id_of, barcode, umi, flags, out);
 }
 
